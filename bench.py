@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py -- the `haphic cluster` hot path on B200: Hi-C pairs/sec through the link-matrix build
+"""bench.py -- the `haphic cluster` hot path on an H100: Hi-C pairs/sec through the link-matrix build
 and MCL iterations/sec, on the synthetic 50k-contig / 200M-pair workload (BASELINE.json configs[2]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
-    python bench.py --impl reference [...]                          # the UNMODIFIED reference (baseline/_ref) on the host cores
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo's CUDA path
+    python bench.py --impl reference [...]                          # the UNMODIFIED reference (oracle/_ref) on the host cores
 
 One "step" = one pass of the hot path over the whole synthetic input:
     link counting (200M records) -> first-seen index -> symmetric CSC -> column normalise ->
@@ -13,6 +13,11 @@ the library's stream); `mcl.value` = MCL iterations/s over the sweep (normalise 
 all iterations, the reference's own definition, HapHiC_cluster.py:2951-2953); `e2e` = the same
 quantities through the public host API with HOST (pinned) buffers, H2D and D2H inside the timed
 region.  Rank 0 prints ONE JSON line.
+
+--dump-outputs DIR writes what the last timed step computed, as a caller of the path receives it, to DIR/<name>.npy
+(float64; fixed seeded samples of the large arrays, under 64 MB in all; single-GPU runs only).  The inputs are generated
+from --seed by torch's generator on the device, whose stream depends on the GPU model (its SM count), so two builds run
+with the same arguments on the same GPU model can be compared output for output.
 """
 
 from __future__ import annotations
@@ -54,7 +59,12 @@ def parse_args():
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--no-default-sweep", action="store_true", help="skip the 20-inflation default sweep figure")
     p.add_argument("--verbose", action="store_true")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the last timed step's outputs to DIR/<name>.npy (float64, at most 64 MB in all)")
+    a = p.parse_args()
+    if a.steps < 1:
+        p.error("--steps must be at least 1")
+    return a
 
 
 def workload_name(a):
@@ -69,7 +79,7 @@ def measured_peaks():
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def measured_tensor_peak():
@@ -80,12 +90,12 @@ def measured_tensor_peak():
             d = json.load(f)
         return float(d["bf16_tflops_sustained"]), float(d["bf16_tflops"]), "measured (MEASURED_PEAKS.json: sustained / burst)"
     except Exception:
-        return 1400.0, 1590.0, "fallback (B200_PROFILING.md)"
+        return 989.0, 989.0, "H100 SXM data sheet (dense bf16 / f16 at 700 W), not measured"
 
 
 def preexp_roofline(pre, n, nnz_m0, ncols, traffic):
     """Roofline of the pre-expansion launch, the dominant kernel of the step.
-    dense engine (hh_k_syrk, tcgen05): tensor bound.  achieved = 16-bit tensor flops the launch issues (2 * 256 * 256 * 64 per
+    dense engine (hh_k_syrk, wgmma): tensor bound.  achieved = 16-bit tensor flops the launch issues (2 * 128 * 128 * 64 per
     tile k-block and pass) / its CUDA-event time (summed over the K chunks when the K range is cut); the algorithmic figure of
     SURVEY.md 8(d) (2 b^3 for the block product, fp32 accuracy needing `passes` 16-bit passes) is reported beside it -- the
     symmetric half is skipped, so issued = passes * b^3.
@@ -95,16 +105,13 @@ def preexp_roofline(pre, n, nnz_m0, ncols, traffic):
         sus, burst, src = measured_tensor_peak()
         ach = pre["flops"] / (pre["gemm_ms"] / 1000.0) / 1e12
         alg = 2.0 * float(n) * float(n) * float(ncols)
-        return {"kernel": "hh_k_syrk<cta_group::{}> (tcgen05.mma + TMA + TMEM; pre-expansion M0*M0 -> dense M1, one launch per step)"
-                .format(pre["cta_group"]), "bound": "tensor", "achieved": ach, "peak": sus, "unit": "TFLOP/s", "frac": ach / sus,
+        return {"kernel": "hh_k_syrk (wgmma + TMA; pre-expansion M0*M0 -> dense M1, one launch per step)", "bound": "tensor", "achieved": ach, "peak": sus, "unit": "TFLOP/s", "frac": ach / sus,
                 "peak_burst": burst, "traffic": traffic.get("hh_k_syrk"), "issued_flops": pre["flops"], "passes": pre["passes"],
                 "algorithmic_flops": alg, "algorithmic_frac_8d": alg / (pre["gemm_ms"] / 1000.0) / (sus * 1e12 / pre["passes"]),
                 "launch_ms": pre["gemm_ms"], "densify_ms": pre["densify_ms"], "clip_correction_ms": pre["clip_ms"],
                 "k_chunks": pre.get("k_chunks", 1),
                 "peak_source": src, "note": "algorithmic_frac_8d = 2 n^2 ncols / t / (peak / passes); above 1 because S = C D C is "
-                "symmetric and only tiles on or above the diagonal are computed.  frac can exceed 1: `peak` is the measured cuBLAS "
-                "bf16 figure on dense data under the power cap, these operand planes are ~95 % zeros (the nominal dense peak is "
-                "2250 TFLOP/s)"}
+                "symmetric and only tiles on or above the diagonal are computed"}
     alg = 8 * nnz_m0 + 4 * n * ncols
     ach = alg / (pre["total_ms"] / 1000.0) / 1e9
     return {"kernel": "hh_k_col<SRC_PRODUCT,EPI_DUMP> (pre-expansion M0*M0 -> dense M1, one launch per step)", "bound": "hbm",
@@ -117,14 +124,18 @@ def cpu_baseline_block(a, asm, rank, in_nx, rec):
     """CPU legs on this box's host cores, bounded samples of the same stream: the unmodified reference's pair loop
     (kind "reference"), and beside it the single-core C port of the same loop (oracle/haphic_oracle.c)."""
     import tempfile
-    n_ref = min(int(rec.shape[0]), a.cpu_sample_pairs)
-    sample = rec[:n_ref].cpu().numpy()
-    with tempfile.TemporaryDirectory() as tmp:
-        v, dt, nnz = ref_pairs_per_sec(asm, sample, tmp)
-    cpu = {"value": v, "unit": "pairs/s", "cores": 1, "kind": "reference",
-           "sample": "first {} records as .pairs text through the unmodified HapHiC_cluster.parse_alignments_for_ctgs("
-                     "pairs_generator_inter_ctgs(...)) from baseline/_ref, {:.1f} s (single-threaded Python by construction; "
-                     "host has {} cores)".format(len(sample), dt, os.cpu_count())}
+    from oracle import refimpl
+    if refimpl.available():
+        n_ref = min(int(rec.shape[0]), a.cpu_sample_pairs)
+        sample = rec[:n_ref].cpu().numpy()
+        with tempfile.TemporaryDirectory() as tmp:
+            v, dt, nnz = ref_pairs_per_sec(asm, sample, tmp)
+        cpu = {"value": v, "unit": "pairs/s", "cores": 1, "kind": "reference",
+               "sample": "first {} records as .pairs text through the unmodified HapHiC_cluster.parse_alignments_for_ctgs("
+                         "pairs_generator_inter_ctgs(...)) from oracle/_ref, {:.1f} s (single-threaded Python by construction; "
+                         "host has {} cores)".format(len(sample), dt, os.cpu_count())}
+    else:
+        cpu = {"kind": "reference", "unavailable": refimpl.MISSING}
     try:
         big = rec[: 8_000_000].cpu().numpy()
         vc, dtc = cpu_c_pairs_per_sec(asm, rank, in_nx, big)
@@ -196,7 +207,7 @@ def cpu_pairs_per_sec(asm, rank, in_nx, sample):
 
 
 def ref_pairs_per_sec(asm, sample, tmp):
-    """The reference's OWN per-read-pair loop, unmodified (baseline/_ref/HapHiC_cluster.py imported by oracle/refimpl.py):
+    """The reference's OWN per-read-pair loop, unmodified (oracle/_ref/HapHiC_cluster.py imported by oracle/refimpl.py):
     parse_alignments_for_ctgs over pairs_generator_inter_ctgs on a .pairs text of the sample (1562-1583, 1596-1655),
     single-threaded by construction.  Returns (pairs/s, seconds, distinct pairs)."""
     from oracle import refimpl
@@ -215,6 +226,8 @@ def ref_mcl_small(a, inflations):
     from haphic_b200.links import name_rank
     from oracle import haphic_oracle as orc
     from oracle import refimpl
+    if not refimpl.available():
+        return {"kind": "reference", "unavailable": refimpl.MISSING}
     small = synth.make_assembly(max(2, a.nchr // 8), 2000, a.mean_len, seed=a.seed)
     sp_pairs = synth.make_pairs(small, min(a.pairs // max(1, a.contigs // 2000), 2_000_000), seed=a.seed + 1).numpy()
     r = orc.count_links_numpy(sp_pairs, small.lengths, name_rank(small.names), np.ones(small.n, np.uint8), 500000)
@@ -314,8 +327,7 @@ def run_reference(a):
     from haphic_b200 import synth
     from oracle import refimpl
     if not refimpl.available():
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref/HapHiC_cluster.py missing (run __graft_entry__.build() "
-                                                                "in the build container)"}))
+        print(json.dumps({"impl": "reference", "unavailable": refimpl.MISSING}))
         return
     asm = synth.make_assembly(a.nchr, a.contigs, a.mean_len, seed=a.seed)
     inflations = [float(x) for x in a.inflations.split(",")]
@@ -349,8 +361,8 @@ def run_reference(a):
 
 
 def ncu_traffic(workload):
-    """DRAM bytes per launch from the committed ncu capture (profiles/traffic.json); only valid for the workload it
-    was captured on."""
+    """DRAM bytes per launch from an optional profiler capture (profiles/traffic.json, not part of the repository); only
+    valid for the workload and device it was captured on."""
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "traffic.json")
     try:
         with open(path) as f:
@@ -360,6 +372,62 @@ def ncu_traffic(workload):
     return t if t.get("workload") == workload else {}
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def write_dumps(path, dump, seed):
+    """The outputs of the last timed step as DIR/<name>.npy, float64.  The large arrays are replaced by the same seeded
+    sample of their rows in every run (in their original order); the sample sizes shrink with the number of inflations
+    so that the files stay under 64 MB."""
+    from haphic_b200.mcl import interpret_result
+
+    n, n_infl = dump["matrix"].shape[0], len(dump["mcl"])
+    small = 8 * n * (1 + n_infl) + (1 << 16)                  # linked index, cluster labels, totals
+    k_links, k_matrix, k_mcl = 500_000, 500_000, 250_000       # sampled rows of 4, 3 and 3 float64 columns
+    sampled = 8 * (4 * k_links + 3 * k_matrix + 3 * k_mcl * n_infl)
+    if small + sampled > DUMP_LIMIT:
+        f = (DUMP_LIMIT - small) / sampled
+        if f <= 0:
+            raise RuntimeError("--dump-outputs: {} contigs x {} inflations do not fit 64 MB".format(n, n_infl))
+        k_links, k_matrix, k_mcl = int(k_links * f), int(k_matrix * f), int(k_mcl * f)
+
+    def rows(n, k):
+        if n <= k:
+            return np.arange(n)
+        return np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False))
+
+    def coo(m):
+        m = m.tocsc()
+        col = np.repeat(np.arange(m.shape[1]), np.diff(m.indptr))
+        return np.stack([m.indices, col, m.data], 1)
+
+    out = {}
+    t = dump["table"]
+    sel = rows(len(t["key_i"]), k_links)
+    out["links_sample"] = np.stack([t["key_i"][sel], t["key_j"][sel], t["full"][sel], t["flank"][sel]], 1)
+    out["links_totals"] = np.array([len(t["key_i"]), t["full"].sum(dtype=np.int64), t["flank"].sum(dtype=np.int64)])
+    out["linked_index"] = dump["index"]
+    m = coo(dump["matrix"])
+    out["matrix_sample"] = m[rows(len(m), k_matrix)]
+    out["matrix_totals"] = np.array([dump["matrix"].shape[0], len(m), m[:, 2].astype(np.float64).sum()])
+    out["mcl_rounds"] = np.array([[r, rounds] for r, rounds, _ in dump["mcl"]])
+    for r, _, fin in dump["mcl"]:
+        tag = "{:g}".format(r).replace(".", "p")
+        f = coo(fin)
+        out["mcl_r{}_sample".format(tag)] = f[rows(len(f), k_mcl)]
+        labels = np.full(fin.shape[0], -1, np.int64)           # cluster of every matrix index, clusters ordered by first member
+        for k, c in enumerate(sorted(interpret_result(fin) or [], key=min)):
+            labels[list(c)] = k
+        out["mcl_r{}_clusters".format(tag)] = labels
+    out = {k: np.ascontiguousarray(v, dtype=np.float64) for k, v in out.items()}
+    total = sum(v.nbytes for v in out.values())
+    if total > DUMP_LIMIT:
+        raise RuntimeError("--dump-outputs: {} bytes exceed the 64 MB budget".format(total))
+    os.makedirs(path, exist_ok=True)
+    for k, v in out.items():
+        np.save(os.path.join(path, k + ".npy"), v)
+
+
 def run_b200(a):
     import torch
 
@@ -367,6 +435,8 @@ def run_b200(a):
     rank_id = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if world > 1:
+        if a.dump_outputs:
+            sys.exit("bench.py: --dump-outputs is supported with one GPU only")
         from haphic_b200 import dist as hdist
         return hdist.bench_multi(a, world, rank_id, local)
 
@@ -389,9 +459,11 @@ def run_b200(a):
     def ev():
         return torch.cuda.Event(enable_timing=True)
 
-    def one_step(timed):
-        """Resident-input pass.  Returns per-stage device times (ms) and statistics."""
+    def one_step(dump=None):
+        """Resident-input pass.  Returns per-stage device times (ms) and statistics.  With a dict `dump` the outputs a
+        caller receives are fetched into it; the fetches are excluded from the stage times and from `excluded_s`."""
         e = [ev() for _ in range(4)]
+        fetch_ms, t_fetch = 0.0, 0.0
         e[0].record(stream)
         tab = LinkTable(ctx, asm.lengths, rank, in_nx, 500000, capacity_hint=hint)
         tab.add(rec, asynchronous=True)
@@ -406,6 +478,15 @@ def run_b200(a):
         per_infl = []
         for r in inflations:
             st = mc.run(r, a.max_iter, a.pruning)
+            if dump is not None:                            # hh_mcl_run has returned: the device is idle
+                t0 = time.perf_counter()
+                f0, f1 = ev(), ev()
+                f0.record(stream)
+                dump["mcl"].append((r, st["rounds"], mc.result()))
+                f1.record(stream)
+                f1.synchronize()
+                fetch_ms += f0.elapsed_time(f1)
+                t_fetch += time.perf_counter() - t0
             iters += st["rounds"]
             kernel_ms += float(st["iter_ms"].sum())
             alg_bytes += st["bytes"]
@@ -415,8 +496,13 @@ def run_b200(a):
                              "ms_iter": [round(float(x), 3) for x in st["iter_ms"][:6]]})
         e[3].record(stream)
         e[3].synchronize()
+        if dump is not None:
+            t0 = time.perf_counter()
+            dump.update(table=tab.fetch(), index=index.copy(), matrix=mat.to_scipy())
+            t_fetch += time.perf_counter() - t0
         out = {
-            "build_ms": e[0].elapsed_time(e[1]), "matrix_ms": e[1].elapsed_time(e[2]), "mcl_ms": e[2].elapsed_time(e[3]),
+            "build_ms": e[0].elapsed_time(e[1]), "matrix_ms": e[1].elapsed_time(e[2]),
+            "mcl_ms": e[2].elapsed_time(e[3]) - fetch_ms, "excluded_s": t_fetch,
             "iters": iters, "kernel_ms": kernel_ms, "alg_bytes": alg_bytes, "products": products,
             "nnz_full": int(info.nnz_full), "nnz_flank": int(info.nnz_flank), "n_used": int(info.n_used),
             "nnz_m0": mc.nnz_m0, "preexp_ms": mc.preexp_ms, "preexp_products": mc.preexp_products,
@@ -428,15 +514,16 @@ def run_b200(a):
         return out
 
     for _ in range(a.warmup):
-        one_step(False)
+        one_step()
     sampler = ClockSampler(0)
     sampler.start()
     l0 = ctx.launches
     torch.cuda.synchronize()
     t_wall0 = time.perf_counter()
-    steps = [one_step(True) for _ in range(a.steps)]
+    dump = {"mcl": []} if a.dump_outputs else None
+    steps = [one_step(dump if k == a.steps - 1 else None) for k in range(a.steps)]
     torch.cuda.synchronize()
-    t_wall = time.perf_counter() - t_wall0
+    t_wall = time.perf_counter() - t_wall0 - sum(s["excluded_s"] for s in steps)
     launches = ctx.launches - l0
     clocks = sampler.stop()
 
@@ -555,12 +642,15 @@ def run_b200(a):
     if not a.no_cpu_baseline and a.ingest_lines > 0:
         ingest = ingest_rate(asm, rec[: a.ingest_lines].cpu().numpy())
 
+    if dump is not None:
+        write_dumps(a.dump_outputs, dump, a.seed)
+
     line = {
         "metric": "hic_pairs_per_sec_matrix_build", "value": pairs_per_s, "unit": "pairs/s", "n_gpus": 1,
         "steps": a.steps, "warmup": a.warmup, "ms_per_step": 1000.0 * t_wall / a.steps, "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "int32 counts / fp32 matrix", "data": "synthetic",
         "config": {"workload": workload_name(a), "inflations": inflations, "max_iter": a.max_iter, "pruning": a.pruning,
-                   "cache": "inputs (16 B x pairs = {:.1f} GB) and the dense pre-expanded matrix exceed the 126 MB L2".format(
+                   "cache": "inputs (16 B x pairs = {:.1f} GB) and the dense pre-expanded matrix exceed the 50 MB L2".format(
                        16 * P / 1e9),
                    "step": "link build + index + CSC + normalise + pre-expansion + MCL sweep"},
         "stage_ms": {"link_build": build_ms, "matrix": matrix_ms, "mcl_sweep": mcl_ms},

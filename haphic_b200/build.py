@@ -1,4 +1,4 @@
-"""Build libhaphic_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libhaphic_b200.so in-tree with nvcc for sm_90a (H100) (cross-compiles without a GPU)."""
 
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libhaphic_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
@@ -34,7 +34,9 @@ def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(HERE, "..", "include", "*.h"))
+    # build.py holds the compiler flags and the target architecture: a library built with other flags is rebuilt
+    deps = (sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(HERE, "..", "include", "*.h"))
+            + [os.path.abspath(__file__)])
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -57,7 +59,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed: {}\n{}".format(" ".join(cmd), out))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-lz"]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + ["-lz"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed: {}\n{}".format(" ".join(cmd), r.stdout))

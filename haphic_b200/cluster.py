@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""`haphic cluster` on the B200 -- a drop-in for scripts/HapHiC_cluster.py of zengxiaofei/HapHiC.
+"""`haphic cluster` on the H100 -- a drop-in for scripts/HapHiC_cluster.py of zengxiaofei/HapHiC.
 
 Same command line, same ``parse_arguments() / run(args, log_file) / main()`` entry points, same
 files written into the working directory (HT_links.pkl, paired_links.clm, full_links.pkl,
@@ -978,8 +978,7 @@ def _ranked_lists(names, c_of, g_of, sums):
 
 def _ranked_group_links_device(link_dict, gid, ng, device):
     """The same ranking with the 2 * nnz directed entries resident on the GPU (torch tensor ops as plumbing: gather, unique,
-    integer index_add, scatter-min, stable sorts; integer arithmetic only, so the result is the numpy path's bit for bit).
-    At 50k contigs / 5.9e7 pairs the host version needs ~10 s per inflation, this one some tens of milliseconds."""
+    integer index_add, scatter-min, stable sorts; integer arithmetic only, so the result is the numpy path's bit for bit)."""
     import torch
     dev = device if isinstance(device, torch.device) else torch.device("cuda", device)
     ctg, oth, val = link_dict.directed_device(dev)
@@ -1267,7 +1266,7 @@ def run(args, log_file=None):
     for flag in ("density_lower", "density_upper", "read_depth_upper", "rank_sum_upper"):
         check_param("--" + flag, getattr(args, flag), {"X", "x"})
     if args.dense_matrix:
-        logger.info("--dense_matrix is set: the pre-expansion runs as a dense GEMM on the tensor cores (tcgen05); "
+        logger.info("--dense_matrix is set: the pre-expansion runs as a dense GEMM on the tensor cores (wgmma); "
                     "the iterates are stored sparsely in either mode")
     if args.aln_format == "auto":
         detect_format(args)

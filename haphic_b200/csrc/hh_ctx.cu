@@ -32,8 +32,8 @@ extern "C" int hh_ctx_create(int device, hh_ctx** out) {
     HH_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     HH_CUDA(cudaGetDeviceProperties(&prop, device));
-    HH_REQUIRE(prop.major >= 10, HH_ERR_UNSUPPORTED,
-               "hh_ctx_create: device %d is sm_%d%d; this library is built for sm_100a (B200) only", device,
+    HH_REQUIRE(prop.major == 9 && prop.minor == 0, HH_ERR_UNSUPPORTED,
+               "hh_ctx_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
                prop.major, prop.minor);
     hh_ctx* c = new (std::nothrow) hh_ctx();
     HH_REQUIRE(c != nullptr, HH_ERR_NOMEM, "hh_ctx_create: out of host memory");

@@ -1,4 +1,4 @@
-// Dense-block pre-expansion on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// Dense-block pre-expansion on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 // What it computes (scripts/HapHiC_cluster.py:2144-2149, dense mode 2035 / 2149): the one-off pre-expansion
 //     M1 = M0 . M0,   M0 = normalize(link_matrix, 'l1', axis=0)
@@ -14,18 +14,9 @@
 //   B = M0     three planes (8 + 8 + 8 significant bits).
 // A bf16 x bf16 product is exact in fp32, so the passes (plane_a, plane_b) below reproduce the fp32 product up to
 // dropped terms of relative size 2^-24.  The accumulation inside the tensor core is not IEEE round-to-nearest, so a
-// tile's K range is cut into chunks: each chunk accumulates in TMEM, is drained by the epilogue warps and added to fp32
-// REGISTER accumulators with round-to-nearest (HH_GEMM_CHUNK k-blocks per chunk).
+// tile's K range is cut into chunks: each chunk accumulates in the wgmma accumulator registers and is then added to a
+// second set of fp32 registers with round-to-nearest (HH_GEMM_CHUNK k-blocks per chunk).
 //
-// Kernel shape (one persistent CTA pair per two SMs, cta_group::2):
-//   tile 256 x 256 (128 rows of A and 128 rows of B per CTA), BLOCK_K = 64 bf16 = one 128-byte swizzle atom;
-//   warp 0   TMA producer: per k-block one 128x64 box per operand plane (cp.async.bulk.tensor, SWIZZLE_128B)
-//            into a ring of shared-memory stages, completion on the LEADER CTA's mbarrier;
-//   warp 1   allocates TMEM; in the leader CTA one thread issues tcgen05.mma (M=256, N=256, K=16) for every pass and
-//            commits to the stage's "empty" barrier (multicast to both CTAs) and to the chunk's "full" barrier;
-//   warps 2-9  epilogue: tcgen05.ld the chunk (32 lanes x 128 columns per warp), add into registers, release the TMEM
-//            buffer; after the last chunk scale and store the tile and its mirror image.
-// HH_GEMM_CG=1 selects a single-CTA variant (tile 128 x 128, cta_group::1) with the same shared-memory layout.
 #include "hh_common.cuh"
 #include "hh_internal.cuh"
 #include "hh_gemm.cuh"
@@ -39,19 +30,6 @@
 // ---------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t hg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ uint32_t hg_cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void hg_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t hg_mapa(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
 __device__ __forceinline__ void hg_mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
@@ -71,109 +49,68 @@ __device__ __forceinline__ void hg_mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void hg_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void hg_mbar_arrive_local(uint32_t bar) {
+__device__ __forceinline__ void hg_mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void hg_mbar_arrive_cluster(uint32_t remote_bar) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote_bar) : "memory");
-}
 
-template <int CG>
 __device__ __forceinline__ void hg_tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t mbar, int c0, int c1, int c2) {
-    if (CG == 2) {
-        asm volatile(
-            "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-            "l"(tm), "r"(mbar), "r"(c0), "r"(c1), "r"(c2)
-            : "memory");
-    } else {
-        asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-                     "l"(tm), "r"(mbar), "r"(c0), "r"(c1), "r"(c2)
-                     : "memory");
-    }
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+                 "l"(tm), "r"(mbar), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
 }
 __device__ __forceinline__ void hg_prefetch_tmap(const CUtensorMap* tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
 
-template <int CG>
-__device__ __forceinline__ void hg_tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    if (CG == 2) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-}
-template <int CG>
-__device__ __forceinline__ void hg_tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    if (CG == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void hg_tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void hg_tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] . B[smem]^T, bf16 operands, fp32 accumulator
-template <int CG>
-__device__ __forceinline__ void hg_umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if (CG == 2) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-// all MMAs issued so far by this thread -> arrive on an mbarrier when they have completed (both CTAs of the pair)
-template <int CG>
-__device__ __forceinline__ void hg_umma_commit(uint32_t bar) {
-    if (CG == 2) {
-        asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                     "h"((uint16_t)3)
-                     : "memory");
-    } else {
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-    }
-}
-// 32 lanes x 32 consecutive columns of TMEM -> 32 registers per thread (lane = TMEM lane, register = column)
-__device__ __forceinline__ void hg_tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void hg_tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// shared-memory matrix descriptor of a K-major tile stored as [rows][64 bf16] with the 128-byte swizzle TMA applies:
-// 8-row groups 1024 bytes apart (SBO), version 1 (Blackwell), layout SWIZZLE_128B.  The start address moves by 32 bytes
-// per K = 16 step inside the swizzle atom.
+// shared-memory matrix descriptor (sm_90 wgmma) of a K-major tile stored as [rows][64 16-bit] with the 128-byte swizzle TMA
+// applies: 8-row groups 1024 bytes apart (SBO), layout type 1 = SWIZZLE_128B.  The start address moves by 32 bytes per K = 16
+// step inside the swizzle atom.
 __device__ __forceinline__ uint64_t hg_make_desc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
     d |= (uint64_t)1 << 16;               // leading byte offset: unused for swizzled K-major layouts
     d |= (uint64_t)(1024 >> 4) << 32;     // stride byte offset
-    d |= (uint64_t)1 << 46;               // descriptor version
-    d |= (uint64_t)2 << 61;               // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;               // SWIZZLE_128B
     return d;
+}
+
+__device__ __forceinline__ void hg_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void hg_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void hg_wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D (+)= A[smem] . B[smem]^T for one warpgroup: M = 64 rows of A, N = 128 rows of B, K = 16, 16-bit operands (bf16 or f16),
+// fp32 accumulator in 64 registers per thread.  accumulate == 0 overwrites D.
+#define HG_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define HG_WGMMA_BODY(TYPES)                                                                                                      \
+    asm volatile(                                                                                                                 \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                                         \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPES " "                                                                  \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                                 \
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                        \
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                         \
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "                                       \
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"                                                                                           \
+        : HG_ACC8(0), HG_ACC8(8), HG_ACC8(16), HG_ACC8(24), HG_ACC8(32), HG_ACC8(40), HG_ACC8(48), HG_ACC8(56)                   \
+        : "l"(adesc), "l"(bdesc), "r"(accumulate))
+template <bool F16>
+__device__ __forceinline__ void hg_wgmma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if (F16) HG_WGMMA_BODY("f16.f16");
+    else HG_WGMMA_BODY("bf16.bf16");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // the GEMM kernel
 // ---------------------------------------------------------------------------------------------------------------------
-#define HG_THREADS 320
-#define HG_PLANE_BYTES 16384        // 128 rows x 64 bf16
+// Kernel shape (one persistent CTA per SM, tile 128 x 128, BLOCK_K = 64 16-bit = one 128-byte swizzle atom):
+//   warpgroup 0      TMA producer (one thread): per k-block one 128x64 box per operand plane (cp.async.bulk.tensor,
+//                    SWIZZLE_128B) into a ring of shared-memory stages, completion on the stage's "full" mbarrier;
+//   warpgroups 1, 2  rows 0-63 / 64-127 of the tile: wgmma (m64n128k16) for every pass and k step into register
+//                    accumulators, then release the stage on its "empty" mbarrier (one arrival per warp).  Every
+//                    HH_GEMM_CHUNK k-blocks the chunk accumulator is added to a second set of fp32 registers with
+//                    round-to-nearest; after the last chunk the tile and its mirror image are scaled and stored.
+#define HG_THREADS 384
+#define HG_TILE 128
+#define HG_PLANE_BYTES 16384        // 128 rows x 64 16-bit elements
 #define HG_MAX_STAGES 4
 
 struct hh_gemm_args {
@@ -183,7 +120,7 @@ struct hh_gemm_args {
     int na, nb;            // planes of A / of B per k-block (1..3)
     int npass;
     int pa[8], pb[8];      // pass list: plane of A, plane of B
-    int chunk_kb;          // k-blocks accumulated in TMEM before they are drained into registers
+    int chunk_kb;          // k-blocks accumulated by the tensor core before they are added into the round-to-nearest registers
     int stages;
     float* m1;             // dense column-major [ld x (col_hi - col_lo)]
     long long ld;
@@ -191,30 +128,16 @@ struct hh_gemm_args {
     const float* inv_s;    // 1 / column sum
     float out_scale;       // applied instead when inv_s == NULL
     int accumulate;        // 1: the epilogue adds to what the output holds (K range processed in several launches)
-    int split_lo;          // 1: passes with a low-order plane accumulate in their own TMEM buffer over the whole tile (see kernel)
-    uint32_t idesc_fmt;    // operand format bits of the instruction descriptor (bit 7: A is bf16, bit 10: B is bf16)
 };
 
-template <int CG, bool SPLIT>
+template <bool F16>
 __global__ void __launch_bounds__(HG_THREADS, 1)
 hh_k_syrk(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const hh_gemm_args a) {
-    constexpr int BN = 128 * CG;              // tile columns (= TMEM columns per accumulator buffer)
-    constexpr int CW = BN / 2;                // columns per epilogue warp
-    constexpr uint32_t TMEM_COLS = 2 * BN;    // two accumulator buffers
-    // kind::f16 descriptor: fp32 accumulator (bit 4), A / B format (bits 7-9 / 10-12: 0 = f16, 1 = bf16), both K-major, N >> 3, M >> 4
-    const uint32_t IDESC = (1u << 4) | a.idesc_fmt | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((128 * CG) >> 4) << 24);
-
     extern __shared__ uint8_t hg_smem_raw[];
     __shared__ __align__(8) uint64_t s_full[HG_MAX_STAGES];
     __shared__ __align__(8) uint64_t s_empty[HG_MAX_STAGES];
-    __shared__ __align__(8) uint64_t s_tfull[2];
-    __shared__ __align__(8) uint64_t s_tempty[2];
-    __shared__ uint32_t s_tmem;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = (CG == 2) ? hg_cluster_ctarank() : 0u;
-    const int pair = (CG == 2) ? (blockIdx.x >> 1) : blockIdx.x;
-    const int npairs = (CG == 2) ? (gridDim.x >> 1) : gridDim.x;
+    const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
     const uint32_t smem_base = (hg_smem_u32(hg_smem_raw) + 1023u) & ~1023u;
     const uint32_t stage_bytes = (uint32_t)(a.na + a.nb) * HG_PLANE_BYTES;
     const int S = a.stages;
@@ -222,43 +145,30 @@ hh_k_syrk(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
             hg_mbar_init(hg_smem_u32(&s_full[s]), 1);
-            hg_mbar_init(hg_smem_u32(&s_empty[s]), 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            hg_mbar_init(hg_smem_u32(&s_tfull[b]), 1);
-            hg_mbar_init(hg_smem_u32(&s_tempty[b]), 8 * CG);     // every epilogue warp of the pair
+            hg_mbar_init(hg_smem_u32(&s_empty[s]), 8);        // every consumer warp
         }
         hg_fence_barrier_init();
         hg_prefetch_tmap(&tmA);
         hg_prefetch_tmap(&tmB);
     }
-    __syncwarp();
-    if (warp == 1) hg_tmem_alloc<CG>(hg_smem_u32(&s_tmem), TMEM_COLS);
-    hg_tc_fence_before();
-    if (CG == 2) hg_cluster_sync();
-    else __syncthreads();
-    hg_tc_fence_after();
-    const uint32_t tmem_base = s_tmem;
+    __syncthreads();
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ------------------------------------------------------------------------------------------- TMA producer
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             int s = 0;
             uint32_t ph = 0;
-            const uint32_t full0 = (CG == 2) ? hg_mapa(hg_smem_u32(&s_full[0]), 0) : hg_smem_u32(&s_full[0]);
-            for (int it = pair; it < a.n_items; it += npairs) {
+            for (int it = blockIdx.x; it < a.n_items; it += gridDim.x) {
                 const hh_gemm_item w = a.items[it];
-                const int rowA = w.m0 + (int)rank * 128;
-                const int rowB = w.n0 + (int)rank * 128;
                 for (int seg = 0; seg < 2; ++seg) {
                     for (int kb = w.kb_lo[seg]; kb < w.kb_hi[seg]; ++kb) {
                         hg_mbar_wait(hg_smem_u32(&s_empty[s]), ph ^ 1u);
-                        if (rank == 0) hg_mbar_expect_tx(hg_smem_u32(&s_full[s]), stage_bytes * CG);
+                        const uint32_t bar = hg_smem_u32(&s_full[s]);
+                        hg_mbar_expect_tx(bar, stage_bytes);
                         const uint32_t dst = smem_base + (uint32_t)s * stage_bytes;
-                        const uint32_t bar = full0 + (uint32_t)s * 8u;
-                        for (int p = 0; p < a.na; ++p) hg_tma_load_3d<CG>(dst + (uint32_t)p * HG_PLANE_BYTES, &tmA, bar, kb * 64, rowA, p);
+                        for (int p = 0; p < a.na; ++p) hg_tma_load_3d(dst + (uint32_t)p * HG_PLANE_BYTES, &tmA, bar, kb * 64, w.m0, p);
                         for (int p = 0; p < a.nb; ++p)
-                            hg_tma_load_3d<CG>(dst + (uint32_t)(a.na + p) * HG_PLANE_BYTES, &tmB, bar, kb * 64, rowB, p);
+                            hg_tma_load_3d(dst + (uint32_t)(a.na + p) * HG_PLANE_BYTES, &tmB, bar, kb * 64, w.n0, p);
                         if (++s == S) {
                             s = 0;
                             ph ^= 1u;
@@ -267,145 +177,93 @@ hh_k_syrk(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 }
             }
         }
-        __syncwarp();     // the other lanes wait here: the teardown barrier is .aligned
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------------------------------- MMA issuer
-        if (rank == 0 && lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            uint32_t g = 0;     // running chunk counter: TMEM buffer g & 1, phase (g >> 1) & 1  (split_lo: buffer 0, phase g & 1)
-            constexpr bool split = SPLIT;       // compiled out of the default kernel
-            for (int it = pair; it < a.n_items; it += npairs) {
-                const hh_gemm_item w = a.items[it];
-                int in_chunk = 0;
-                const int total = (w.kb_hi[0] - w.kb_lo[0]) + (w.kb_hi[1] - w.kb_lo[1]);
-                for (int t = 0; t < total; ++t) {
-                    const uint32_t buf = split ? 0u : (g & 1u);
-                    if (in_chunk == 0) {
-                        hg_mbar_wait(hg_smem_u32(&s_tempty[buf]), (split ? (g & 1u) : ((g >> 1) & 1u)) ^ 1u);
-                        hg_tc_fence_after();
-                    }
-                    hg_mbar_wait(hg_smem_u32(&s_full[s]), ph);
-                    hg_tc_fence_after();
-                    const uint32_t st = smem_base + (uint32_t)s * stage_bytes;
-                    const uint32_t d_hi = tmem_base + buf * (uint32_t)BN;
-                    const uint32_t d_lo = tmem_base + (uint32_t)BN;
-                    uint32_t hi_acc = in_chunk ? 1u : 0u, lo_acc = t ? 1u : 0u;      // 0: the MMA overwrites the accumulator
-                    for (int p = 0; p < a.npass; ++p) {
-                        const uint64_t ad = hg_make_desc(st + (uint32_t)a.pa[p] * HG_PLANE_BYTES);
-                        const uint64_t bd = hg_make_desc(st + (uint32_t)(a.na + a.pb[p]) * HG_PLANE_BYTES);
-                        const bool lo = split && (a.pa[p] | a.pb[p]) != 0;
+        return;
+    }
+
+    // ----------------------------------------------------------------------------------------------- consumers
+    const int e = wg - 1;                          // rows 64 e .. 64 e + 63 of the tile
+    const int wq = (threadIdx.x >> 5) & 3;         // warp within the warpgroup
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[64], racc[64];
+    for (int it = blockIdx.x; it < a.n_items; it += gridDim.x) {
+        const hh_gemm_item w = a.items[it];
+        const int total = (w.kb_hi[0] - w.kb_lo[0]) + (w.kb_hi[1] - w.kb_lo[1]);
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            if (lo) {
-                                hg_umma<CG>(d_lo, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC, lo_acc);
-                                lo_acc = 1u;
-                            } else {
-                                hg_umma<CG>(d_hi, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC, hi_acc);
-                                hi_acc = 1u;
-                            }
-                        }
-                    }
-                    hg_umma_commit<CG>(hg_smem_u32(&s_empty[s]));      // the stage is free once these MMAs have read it
-                    if (++s == S) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                    if (++in_chunk == a.chunk_kb || t + 1 == total) {
-                        hg_umma_commit<CG>(hg_smem_u32(&s_tfull[buf]));    // chunk complete -> epilogue
-                        in_chunk = 0;
-                        ++g;
-                    }
-                }
+        for (int j = 0; j < 64; ++j) {
+            acc[j] = 0.f;
+            racc[j] = 0.f;
+        }
+        int in_chunk = 0;
+        for (int t = 0; t < total; ++t) {
+            hg_mbar_wait(hg_smem_u32(&s_full[s]), ph);
+            const uint32_t st = smem_base + (uint32_t)s * stage_bytes;
+            hg_wgmma_fence();
+            for (int p = 0; p < a.npass; ++p) {
+                const uint64_t ad = hg_make_desc(st + (uint32_t)a.pa[p] * HG_PLANE_BYTES + (uint32_t)e * (64u * 128u));
+                const uint64_t bd = hg_make_desc(st + (uint32_t)(a.na + a.pb[p]) * HG_PLANE_BYTES);
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    hg_wgmma<F16>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (in_chunk | p | k) ? 1u : 0u);
+            }
+            hg_wgmma_commit();
+            hg_wgmma_wait0();
+            __syncwarp();
+            if (lane == 0) hg_mbar_arrive(hg_smem_u32(&s_empty[s]));      // this warp's reads of the stage are complete
+            if (++s == S) {
+                s = 0;
+                ph ^= 1u;
+            }
+            if (++in_chunk == a.chunk_kb || t + 1 == total) {
+#pragma unroll
+                for (int j = 0; j < 64; ++j) racc[j] = __fadd_rn(racc[j], acc[j]);
+                in_chunk = 0;
             }
         }
-        __syncwarp();
-    } else {
-        // ------------------------------------------------------------------------------------------- epilogue
-        const int e = warp - 2;
-        const int quarter = warp & 3;          // TMEM lanes this warp may touch: 32 * (warp id % 4)
-        const int half = e >> 2;               // column half of the tile
-        const uint32_t lane_addr = ((uint32_t)(quarter * 32) << 16) + (uint32_t)(half * CW);
-        const uint32_t tempty0 = (CG == 2) ? hg_mapa(hg_smem_u32(&s_tempty[0]), 0) : hg_smem_u32(&s_tempty[0]);
-        uint32_t g = 0;
-        constexpr bool split = SPLIT;
-        float acc[CW];
-        for (int it = pair; it < a.n_items; it += npairs) {
-            const hh_gemm_item w = a.items[it];
-            const int total = (w.kb_hi[0] - w.kb_lo[0]) + (w.kb_hi[1] - w.kb_lo[1]);
-            const int nchunks = (total + a.chunk_kb - 1) / a.chunk_kb;
+        // ---- scale and store: out[r, c] = D * scale[c]; mirror image out[c, r] = D * scale[r].
+        // Accumulator layout of m64nN: register 4 q + 2 h + b holds row 16 wq + lane / 4 + 8 h, column 8 q + 2 (lane % 4) + b.
 #pragma unroll
-            for (int j = 0; j < CW; ++j) acc[j] = 0.f;
-            for (int ch = 0; ch < nchunks; ++ch, ++g) {
-                const uint32_t buf = split ? 0u : (g & 1u);
-                hg_mbar_wait(hg_smem_u32(&s_tfull[buf]), split ? (g & 1u) : ((g >> 1) & 1u));
-                hg_tc_fence_after();
-                // split_lo: after the last chunk of the tile the low-order accumulator (second buffer) is added as well
-                const int nsrc = (split && ch + 1 == nchunks) ? 2 : 1;
-                for (int src = 0; src < nsrc; ++src) {
-                    const uint32_t tb = tmem_base + (src ? (uint32_t)BN : buf * (uint32_t)BN) + lane_addr;
+        for (int h = 0; h < 2; ++h) {
+            const int r = w.m0 + 64 * e + 16 * wq + (lane >> 2) + 8 * h;
+            if (r >= w.m_end) continue;
+            if (w.flags & HH_GEMM_DIRECT) {
+                float* __restrict__ dst = a.m1 + (ptrdiff_t)(r - w.out_row0);
 #pragma unroll
-                    for (int q = 0; q < CW / 32; ++q) {
-                        uint32_t v[32];
-                        hg_tmem_ld32(tb + (uint32_t)(q * 32), v);
-                        hg_tmem_ld_wait();
+                for (int q = 0; q < 16; ++q) {
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[q * 32 + j] = __fadd_rn(acc[q * 32 + j], __uint_as_float(v[j]));
-                    }
-                }
-                hg_tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {
-                    if (CG == 2) hg_mbar_arrive_cluster(tempty0 + buf * 8u);
-                    else hg_mbar_arrive_local(tempty0 + buf * 8u);
-                }
-            }
-            // ---- scale and store: out[r, c] = D * scale[c]; mirror image out[c, r] = D * scale[r]
-            const int r = w.m0 + (int)rank * 128 + quarter * 32 + lane;
-            const int c0 = w.n0 + half * CW;
-            if (r < w.m_end) {
-                if (w.flags & HH_GEMM_DIRECT) {
-                    float* __restrict__ dst = a.m1 + (ptrdiff_t)(r - w.out_row0);
-#pragma unroll
-                    for (int j = 0; j < CW; ++j) {
-                        const int c = c0 + j;
+                    for (int b = 0; b < 2; ++b) {
+                        const int c = w.n0 + 8 * q + 2 * (lane & 3) + b;
                         if (c < w.n_end && c >= a.col_lo && c < a.col_hi) {
                             float* __restrict__ o = dst + (size_t)(c - a.col_lo) * (size_t)a.ld;
-                            const float v = a.inv_s ? acc[j] * __ldg(a.inv_s + c) : acc[j] * a.out_scale;
+                            const float x = racc[4 * q + 2 * h + b];
+                            const float v = a.inv_s ? x * __ldg(a.inv_s + c) : x * a.out_scale;
                             *o = a.accumulate ? __fadd_rn(*o, v) : v;
                         }
                     }
                 }
-                if ((w.flags & HH_GEMM_MIRROR) && r >= a.col_lo && r < a.col_hi) {
-                    const float sr = a.inv_s ? __ldg(a.inv_s + r) : a.out_scale;
-                    float* __restrict__ dst = a.m1 + (size_t)(r - a.col_lo) * (size_t)a.ld - (ptrdiff_t)w.out_row0;
+            }
+            if ((w.flags & HH_GEMM_MIRROR) && r >= a.col_lo && r < a.col_hi) {
+                const float sr = a.inv_s ? __ldg(a.inv_s + r) : a.out_scale;
+                float* __restrict__ dst = a.m1 + (size_t)(r - a.col_lo) * (size_t)a.ld - (ptrdiff_t)w.out_row0;
 #pragma unroll
-                    for (int j = 0; j < CW; j += 4) {
-                        const int c = c0 + j;
-                        if (c + 3 < w.n_end && w.out_row0 == 0) {
-                            float4 v = make_float4(acc[j] * sr, acc[j + 1] * sr, acc[j + 2] * sr, acc[j + 3] * sr);
-                            if (a.accumulate) {
-                                const float4 old = *reinterpret_cast<const float4*>(dst + c);
-                                v = make_float4(__fadd_rn(old.x, v.x), __fadd_rn(old.y, v.y), __fadd_rn(old.z, v.z), __fadd_rn(old.w, v.w));
-                            }
-                            *reinterpret_cast<float4*>(dst + c) = v;
-                        } else {
-#pragma unroll
-                            for (int q = 0; q < 4; ++q)
-                                if (c + q < w.n_end) dst[c + q] = a.accumulate ? __fadd_rn(dst[c + q], acc[j + q] * sr) : acc[j + q] * sr;
+                for (int q = 0; q < 16; ++q) {
+                    const int c = w.n0 + 8 * q + 2 * (lane & 3);
+                    const float v0 = racc[4 * q + 2 * h] * sr, v1 = racc[4 * q + 2 * h + 1] * sr;
+                    if (c + 1 < w.n_end && w.out_row0 == 0) {
+                        float2 v = make_float2(v0, v1);
+                        if (a.accumulate) {
+                            const float2 old = *reinterpret_cast<const float2*>(dst + c);
+                            v = make_float2(__fadd_rn(old.x, v.x), __fadd_rn(old.y, v.y));
                         }
+                        *reinterpret_cast<float2*>(dst + c) = v;
+                    } else {
+                        if (c < w.n_end) dst[c] = a.accumulate ? __fadd_rn(dst[c], v0) : v0;
+                        if (c + 1 < w.n_end) dst[c + 1] = a.accumulate ? __fadd_rn(dst[c + 1], v1) : v1;
                     }
                 }
             }
         }
     }
-
-    // ---- teardown: every MMA has completed (the epilogues consumed the last chunk), free TMEM
-    hg_tc_fence_before();
-    if (CG == 2) hg_cluster_sync();
-    else __syncthreads();
-    hg_tc_fence_after();
-    if (warp == 1) hg_tmem_dealloc<CG>(tmem_base, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -548,37 +406,22 @@ static int hg_env_int(const char* name, int dflt) {
     return (v && *v) ? atoi(v) : dflt;
 }
 
-template <int CG, bool SPLIT>
+template <bool F16>
 static int hg_launch(hh_ctx* ctx, const CUtensorMap& tmA, const CUtensorMap& tmB, const hh_gemm_args& a, size_t smem) {
-    auto kern = hh_k_syrk<CG, SPLIT>;
+    auto kern = hh_k_syrk<F16>;
     HH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    int pairs = ctx->sm_count / CG;
-    if (pairs > a.n_items) pairs = a.n_items;
-    if (pairs < 1) pairs = 1;
-    cfg.gridDim = dim3((unsigned)(pairs * CG));
-    cfg.blockDim = dim3(HG_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    HH_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, a));
-    ctx->launches++;
+    int grid = ctx->sm_count;
+    if (grid > a.n_items) grid = a.n_items;
+    if (grid < 1) grid = 1;
+    HH_LAUNCH(ctx, kern, grid, HG_THREADS, smem, tmA, tmB, a);
     return HH_OK;
 }
 
-int hh_gemm_cta_group() { return hg_env_int("HH_GEMM_CG", 2) == 1 ? 1 : 2; }
-
 int hh_gemm_run(hh_ctx* ctx, const hh_gemm_operand& A, const hh_gemm_operand& B, const hh_gemm_item* d_items, int n_items, int npass,
                 const int* pa, const int* pb, int chunk_kb, float* out, long long ld, int col_lo, int col_hi, const float* scale,
-                int* stages_out, float out_scale, int split_lo, int accumulate) {
+                int* stages_out, float out_scale, int accumulate) {
     HH_REQUIRE(n_items >= 1 && npass >= 1 && npass <= 8, HH_ERR_ARG, "hh_gemm_run: bad work list");
+    HH_REQUIRE(A.fmt == B.fmt, HH_ERR_ARG, "hh_gemm_run: wgmma takes one 16-bit format for both operands");
     CUtensorMap tmA, tmB;
     HH_CHECK(hg_encode(&tmA, (void*)A.base, A.rows, A.kdim, A.ldk, A.plane, A.planes, A.fmt));
     HH_CHECK(hg_encode(&tmB, (void*)B.base, B.rows, B.kdim, B.ldk, B.plane, B.planes, B.fmt));
@@ -593,7 +436,7 @@ int hh_gemm_run(hh_ctx* ctx, const hh_gemm_operand& A, const hh_gemm_operand& B,
         a.pa[p] = pa[p];
         a.pb[p] = pb[p];
     }
-    a.chunk_kb = chunk_kb < 1 ? (1 << 30) : chunk_kb;           // 0 = accumulate the whole K range in TMEM
+    a.chunk_kb = chunk_kb < 1 ? (1 << 30) : chunk_kb;           // 0 = accumulate the whole K range in the tensor core
     const size_t stage_bytes = (size_t)(A.planes + B.planes) * HG_PLANE_BYTES;
     int stages = (int)((ctx->smem_optin - 2048) / stage_bytes);
     if (stages > HG_MAX_STAGES) stages = HG_MAX_STAGES;
@@ -606,12 +449,9 @@ int hh_gemm_run(hh_ctx* ctx, const hh_gemm_operand& A, const hh_gemm_operand& B,
     a.col_hi = col_hi;
     a.inv_s = scale;
     a.out_scale = out_scale;
-    a.split_lo = split_lo;
     a.accumulate = accumulate;
-    a.idesc_fmt = (A.fmt == HH_GEMM_BF16 ? (1u << 7) : 0u) | (B.fmt == HH_GEMM_BF16 ? (1u << 10) : 0u);
     const size_t smem = (size_t)stages * stage_bytes + 1024;
-    if (hh_gemm_cta_group() == 2) return split_lo ? hg_launch<2, true>(ctx, tmA, tmB, a, smem) : hg_launch<2, false>(ctx, tmA, tmB, a, smem);
-    return split_lo ? hg_launch<1, true>(ctx, tmA, tmB, a, smem) : hg_launch<1, false>(ctx, tmA, tmB, a, smem);
+    return A.fmt == HH_GEMM_F16 ? hg_launch<true>(ctx, tmA, tmB, a, smem) : hg_launch<false>(ctx, tmA, tmB, a, smem);
 }
 
 static const int HG_P1[3][2] = {{0, 0}, {0, 1}, {0, 2}};
@@ -657,7 +497,7 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
         // two passes, clip 2048; the excess over `clip` is the caller's sparse correction.  It needs column sums below 2^23 (the
         // scaled counts may be f16 subnormals, exact down to 2^-24).  Otherwise, or with HH_GEMM_FMT=bf16, the exact encoding:
         // one bf16 plane of min(count, 256) against three bf16 planes of M0, three passes.  (kind::f16 takes ONE format for both
-        // operands: a bf16 count plane against f16 planes of M0 is an illegal instruction on sm_100a -- measured.)
+        // operands.)
         // Anything else (weights of --normalize_by_nlinks, allele-aware scaling): three exact bf16 planes each, six passes.
         const char* fmt_env = getenv("HH_GEMM_FMT");
         int enc = 2;                                             // 0 = exact bf16, 2 = scaled f16
@@ -671,11 +511,11 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
             clip = 3.0e38f;
         }
         const int fmt_a = enc == 2 ? HH_GEMM_F16 : HH_GEMM_BF16, fmt_b = enc ? HH_GEMM_F16 : HH_GEMM_BF16;
-        // The K range is cut into equal chunks when the operand planes of the whole range would exceed ~36 GB (150k contigs:
-        // 135 GB): planes of one chunk at a time, the epilogue of every chunk after the first adds to M1.  The cut depends on
+        // The K range is cut into equal chunks when the operand planes of the whole range would exceed ~16 GB (a fifth of an
+        // 80 GB device; 150k contigs: 135 GB): planes of one chunk at a time, the epilogue of every chunk after the first adds to M1.  The cut depends on
         // n and the encoding only, so every rank of a sharded run cuts alike and M1 stays bit-identical for any world size.
         const double plane_bytes_all = (double)(na + nb) * (double)plane * 2.0;
-        int kchunks = (int)(plane_bytes_all / 36.0e9) + 1;
+        int kchunks = (int)(plane_bytes_all / 16.0e9) + 1;
         kchunks = hg_env_int("HH_GEMM_KCHUNKS", kchunks);
         if (kchunks < 1) kchunks = 1;
         const long long kw = ((((long long)n + kchunks - 1) / kchunks) + 63) & ~63ll;      // chunk width, multiple of 64
@@ -696,18 +536,11 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
         }
         const int np_env = hg_env_int("HH_GEMM_NPASS", 0);      // experiments only: fewer passes = lower precision
         if (np_env >= 1 && np_env < npass) npass = np_env;
-        // k-blocks accumulated in TMEM between two drains: the tensor core's accumulate truncates, so the bias grows with the
-        // number of accumulations (4 MMAs per k-block and pass).
-        // Measured at 50k contigs (one B200; GEMM time / max and mean relative error against the exact product), two f16 passes:
-        //   chunk 2: 205 ms, 1.5e-6, -1.6e-8   4: 177 ms, 1.2e-6, -2.4e-8   8: 139 ms, 1.1e-6, -3.9e-8   16: 136 ms, 1.9e-6, -6.6e-8
-        // every drain costs 0.5-2k clocks of tensor-pipe time, so longer chunks are faster -- but on dense inputs (every product
-        // of similar size) the bias of 64 truncating accumulations reaches 2.5e-6.  Three k-blocks = 24 accumulations, the
-        // same as three bf16 passes drained every second k-block, keeps every test input below 2e-6.
-        // HH_GEMM_SPLIT=1 (experiment): the low-order pass (2^-11 of the result) gets the second TMEM buffer for the whole
-        // tile and only the high-order pass is chunked -- bias-free (mean -1.4e-10) but single-buffered: 244 ms against 211 ms
-        // at chunk 8 on the same device.
-        const int split = (enc && hg_env_int("HH_GEMM_SPLIT", 0)) ? 1 : 0;
-        const int chunk = hg_env_int("HH_GEMM_CHUNK", npass > 3 ? 1 : (npass == 3 ? 2 : (split ? 8 : 3)));
+        // k-blocks accumulated by the tensor core between two drains into the round-to-nearest registers: the tensor core's
+        // accumulate truncates, so the bias grows with the number of accumulations (4 MMAs per k-block and pass); on dense
+        // inputs (every product of similar size) 64 truncating accumulations reach 2.5e-6 of relative error.  Three k-blocks
+        // = 24 accumulations, the same as three bf16 passes drained every second k-block, keeps every test input below 2e-6.
+        const int chunk = hg_env_int("HH_GEMM_CHUNK", npass > 3 ? 1 : (npass == 3 ? 2 : 3));
         int stages = 0;
         float densify_ms = 0.f, gemm_ms = 0.f;
         const float stats_ms = 0.f;                              // column sums + value statistics: a fraction of a millisecond
@@ -732,7 +565,7 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
             hh_gemm_operand A = {d_A, na, n, (int)(k1 - k0), kw, plane_c, fmt_a};
             hh_gemm_operand B = {d_B, nb, n, (int)(k1 - k0), kw, plane_c, fmt_b};
             HH_CUDA(cudaEventRecord(ev[1], ctx->stream));
-            HH_CHECK(hh_gemm_run(ctx, A, B, d_items, n_items, npass, pa, pb, chunk, d_m1, ld, col_lo, col_hi, d_inv, &stages, 1.0f, split,
+            HH_CHECK(hh_gemm_run(ctx, A, B, d_items, n_items, npass, pa, pb, chunk, d_m1, ld, col_lo, col_hi, d_inv, &stages, 1.0f,
                                  kc > 0 ? 1 : 0));
             HH_CUDA(cudaEventRecord(ev[2], ctx->stream));
             HH_CUDA(cudaStreamSynchronize(ctx->stream));         // items_c is rewritten for the next chunk
@@ -753,7 +586,7 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
             st->fmt_b = fmt_b;
             st->b_planes = nb;
             st->passes = npass;
-            st->cta_group = hh_gemm_cta_group();
+            st->cta_group = 1;                                   // one CTA per tile
             st->stages = stages;
             st->chunk_kb = chunk < 1 ? (1 << 30) : chunk;
             st->densify_ms = densify_ms + stats_ms;
@@ -761,7 +594,7 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
             st->k_chunks = kchunks;
             double kb = 0.0;
             for (int i = 0; i < n_items; ++i) kb += (double)((h_items[i].kb_hi[0] - h_items[i].kb_lo[0]) + (h_items[i].kb_hi[1] - h_items[i].kb_lo[1]));
-            const double tile = 128.0 * hh_gemm_cta_group();
+            const double tile = (double)HG_TILE;
             st->flops = 2.0 * tile * tile * 64.0 * kb * (double)npass;
         }
         return HH_OK;
@@ -876,7 +709,7 @@ int hh_gemm_blk_operands(hh_ctx* ctx, const int* d_len, const void* d_ent, int c
     return HH_OK;
 }
 
-int hh_gemm_tile_size() { return 128 * (hg_env_int("HH_GEMM_CG", 2) == 1 ? 1 : 2); }
+int hh_gemm_tile_size() { return HG_TILE; }
 
 // work list of the whole-matrix product: every tile pair (a <= b) on or above the diagonal whose result (columns of
 // tile b) or mirror image (columns of tile a) falls into the owned column block [col_lo, col_hi).  A column shard
@@ -891,11 +724,11 @@ int hh_gemm_items_full(int n, int col_lo, int col_hi, std::vector<hh_gemm_item>&
         const int c0 = t * T, c1 = std::min(n, c0 + T);
         return c1 > col_lo && c0 < col_hi;
     };
-    // Rasterisation.  Item i runs on CTA pair (i mod pairs), so `pairs` consecutive items form a wave that streams its
-    // operand panels together: the wave should be a compact block of tiles.  A panels (one bf16 plane) are three times
-    // cheaper than B panels (three planes), so super-blocks are SB_M = 15 tiles tall and SB_N = 5 wide (75 tiles ~ one
-    // wave of 74 pairs): per k-block a wave then reads 15 + 3 * 5 = 30 panel blocks instead of 1 + 3 * 74.
-    const int SB_M = 15, SB_N = 5;
+    // Rasterisation.  Item i runs on CTA (i mod CTAs), so one item per SM (132 on an H100) form a wave that streams its
+    // operand panels together: the wave should be a compact block of tiles.  A panels (one plane) are two to three times
+    // cheaper than B panels (two or three planes), so super-blocks are SB_M = 16 tiles tall and SB_N = 8 wide (128 tiles ~
+    // one wave): per k-block a wave then reads 16 + 2 * 8 = 32 panel blocks instead of 1 + 2 * 132.
+    const int SB_M = 16, SB_N = 8;
     for (int bb = 0; bb < nt; bb += SB_N) {
         for (int ba = 0; ba <= std::min(nt - 1, bb + SB_N - 1); ba += SB_M) {
             for (int ta = ba; ta < std::min(nt, ba + SB_M); ++ta) {

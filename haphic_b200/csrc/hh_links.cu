@@ -26,8 +26,6 @@ struct __align__(32) hh_slot {
 };
 
 // Counter updates of one (warp-aggregated) group of records on a slot: plain 32-bit reductions (fire and forget).
-// (Measured at 200M records: packing full|flank and ht|th into 64-bit adds and guarding the two minima with a load made the
-// counting 7 % slower, not faster -- the launches are not bound by the atomics of hot pairs.)
 __device__ __forceinline__ void hh_slot_update(hh_slot* v, unsigned c_full, unsigned c_fl, uint32_t first_all, uint32_t first_fl,
                                                unsigned c_ht, unsigned c_th, unsigned c_tt) {
     atomicAdd(&v->full, c_full);
@@ -274,8 +272,8 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 // Partition, then aggregate.  One big hash table costs every record a random DRAM sector for the key and another
 // read-modify-write for the counters (the table is two orders of magnitude larger than L2).  For long streams the
 // records are therefore first split by the high bits of the key hash into 2^npart_log partitions (one sequential read,
-// one write in runs that fill whole sectors), and every partition is then counted in a scratch table small enough to
-// stay in L2 and emitted as compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only:
+// one write in runs that fill whole sectors), and every partition is then counted in a scratch table of a few tens of
+// MB (mostly L2 hits; see links_choose_mode for its size on an H100) and emitted as compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only:
 // the result is identical to the direct path.
 //   hh_k_part_scatter   record -> {i, j, stream index, flags} (ends ordered by name rank, is_flank / head-tail evaluated once)
 //   hh_k_part_step      emit + clear the scratch table of the previous partition, count the current one into the other
@@ -955,7 +953,10 @@ static int links_choose_mode(hh_links* lk, int64_t total) {
     }
     lk->mode = 2;
     int lg = 4;
-    while (lg < 9 && ((int64_t)400000 << lg) < total) lg++;            // ~400k records per partition, at most 512 partitions
+    // ~400k records per partition, at most 512 partitions.  At 200M records the two scratch tables (2 x 2^20 slots, 42 MB
+    // each) exceed the H100's 50 MB L2; 1024 partitions (2 x 21 MB, inside L2) were measured slower on an H100 SXM:
+    // link build 46.3 ms against 42.4-42.8 ms -- a step is a latency chain, not bound by where the table lives
+    while (lg < 9 && ((int64_t)400000 << lg) < total) lg++;
     lk->npart_log = links_env_int("HH_LINKS_NPART_LOG", lg);
     if (lk->npart_log < 1) lk->npart_log = 1;
     if (lk->npart_log > 10) lk->npart_log = 10;
@@ -1069,7 +1070,7 @@ extern "C" int hh_links_add(hh_links* lk, const int32_t* rec, int64_t n_rec, int
     return HH_OK;
 }
 
-// partitioned counting, second phase: every partition through an L2-resident scratch table (two tables, so the emit of
+// partitioned counting, second phase: every partition through a small scratch table (two tables, so the emit of
 // partition p - 1 and the count of partition p share one launch), entries appended to an unordered compact list
 static void links_free_partsets(hh_links* lk) {
     if (lk->psets) {

@@ -1716,14 +1716,13 @@ __device__ __noinline__ float hh_it0_x1(float x, double S1, float rf, int sq) {
     return (float)((double)y / S1);
 }
 
-// NW warps per CTA and 32 / NW CTAs per SM.  With 8-warp CTAs 592 columns (118 MB, the whole L2) are in flight and ncu shows
-// all three passes in DRAM (29.6 GB read, L2 hit 4 %) -- but fewer, larger CTAs (59 / 30 MB in flight) are not faster:
-// 10.1 / 10.5 / 11.6 ms for NW = 8 / 16 / 32 at r = 2.0 on the same device.  The kernel is bound by instruction issue
-// (1.0e10 warp instructions, issue slots 61 % busy), not by where the re-reads come from.  HH_MCL_IT0_WARPS selects the shape.
+// NW warps per CTA and 32 / NW CTAs per SM.  With 8-warp CTAs more columns are in flight than L2 holds, so passes 2 and 3
+// re-read from DRAM; fewer, larger CTAs keep the re-reads in L2 but were not faster, because the kernel is bound by
+// instruction issue, not by where the re-reads come from.  HH_MCL_IT0_WARPS selects the shape.
 // QUEUE: the candidates of passes 2 and 3 (a few percent of the elements) are first collected in a per-warp shared-memory
 // queue and then evaluated 32 at a time.  Evaluating them where they are found costs one call of hh_it0_x1 (pow + fp64
 // division, ~100 instructions) per warp and element slot that holds at least one candidate -- with 1-2 % candidates that
-// is every second slot, executed with one or two active lanes: 7.5e9 of the kernel's 1.0e10 warp instructions (ncu).
+// is every second slot, executed with one or two active lanes: most of the kernel's warp instructions.
 template <int W, bool SQ, int NW, bool QUEUE>      // SQ: any of the multiplicative modes (no powf in the streaming loop)
 __global__ void __launch_bounds__(NW * 32, 32 / NW) hh_k_iter0(const hh_colargs a) {
     constexpr int HH_IT0_WARPS = NW;
@@ -2059,8 +2058,7 @@ static int grid_cap_for(hh_ctx* ctx, const hh_geom& g, int* out) {
 // ---------------------------------------------------------------------------------------------
 // Unsorted CSC column -> row-sorted slot without an n-row accumulator: the rows present are marked in a bitmap (n bits of
 // shared memory), an exclusive prefix over the bitmap words gives every row its rank, and every entry writes itself to its
-// rank.  d marks + n/32 words scanned + d lookups per column, instead of 2 n rows scanned (the accumulator kernel spent
-// 13 ms here at 50k contigs).  Column sum in fp64 (sklearn normalize, 2144; exact in any order for integer link counts, the
+// rank.  d marks + n/32 words scanned + d lookups per column, instead of 2 n rows scanned by the accumulator kernel.  Column sum in fp64 (sklearn normalize, 2144; exact in any order for integer link counts, the
 // order below is fixed).  A row stored twice in one column (only a caller's own CSC can have that) raises *dup: the caller
 // then runs the accumulator kernel, which adds duplicates up.
 // ---------------------------------------------------------------------------------------------
@@ -2407,8 +2405,8 @@ static void mcl_base_args(hh_mcl* mc, hh_colargs& a) {
     a.l2pf = mc->l2pf > 0 ? 1 : 0;
 }
 
-// mean entries per (column, row block) segment below which the flat walk beats the segment-wise one
-// (measured on B200, 50k contigs: 32 -> segment-wise 180 ms vs flat 267 ms; 12 -> 71 ms vs 61 ms)
+// mean entries per (column, row block) segment below which the flat walk beats the segment-wise one (at 50k contigs:
+// segment-wise wins at 32 entries per segment, the flat walk at 12)
 static int choose_flat(const hh_mcl* mc, double nnz_operand) {
     if (mc->flat >= 0) return mc->flat > 0;
     const double seg = nnz_operand / (double)mc->n / (double)mc->W;
@@ -2443,23 +2441,24 @@ static int choose_preexp(const hh_matrix* m, int requested) {
         if (!strcmp(e, "dense")) return HH_PREEXP_DENSE;
     }
     if (requested == HH_PREEXP_SPARSE || requested == HH_PREEXP_DENSE) return requested;
-    // measured on B200: Gustavson ~0.5e12 products/s; tensor-core GEMM ~1.9e15 flop/s issued over two f16 passes of the
-    // symmetric half, plus operand planes (memset + scatter) and allocation
+    // cost model in seconds, fitted on one H100 SXM (400 W power limit): the Gustavson engine did n d^2 = 2.7e11 / 3.0e10
+    // products in 1219 / 103 ms at C3 / C2 (0.23e12 / 0.29e12 per second); the two-pass f16 GEMM took 862 ms at n = 49,992
+    // (6.9e-15 n^3) plus 7.6 ms of operand planes (3e-12 n^2).  Both engines meet the same accuracy bar: a speed decision.
     const double n = (double)m->n, d = (double)m->nnz / (n > 0 ? n : 1.0);
-    // (above 57,600 vertices the column accumulator no longer fits shared memory: measured 8.5 s per rank for 1/8 of the
-    // columns at 150k contigs / 1B pairs, about ten times the shared-memory rate)
-    const double t_sparse = n * d * d / (n > 57600.0 ? 0.05e12 : 0.5e12);
-    const double t_dense = 1.2e-15 * n * n * n + 3.0e-12 * n * n + 5.0e-4;
+    // (above 57,600 vertices the column accumulator no longer fits shared memory and the Gustavson engine runs on a global
+    // accumulator; taken as ten times slower, not measured on the H100)
+    const double t_sparse = n * d * d / (n > 57600.0 ? 0.025e12 : 0.25e12);
+    const double t_dense = 6.9e-15 * n * n * n + 3.0e-12 * n * n + 5.0e-4;
     // the operand planes (up to six bf16 planes of n x n) must fit beside M1 and the iterates
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
         cudaGetLastError();
         free_b = 0;
     }
-    // the operand planes of one K chunk (hh_gemm_preexpand cuts the K range so that a chunk stays below ~36 GB; six bf16
+    // the operand planes of one K chunk (hh_gemm_preexpand cuts the K range so that a chunk stays below ~16 GB; six bf16
     // planes in the worst case) must fit beside M1 and the iterates
     const double planes_all = 6.0 * 2.0 * n * n;
-    const double planes = planes_all / (double)((int)(planes_all / 36.0e9) + 1);
+    const double planes = planes_all / (double)((int)(planes_all / 16.0e9) + 1);
     if (planes > 0.5 * (double)free_b) return HH_PREEXP_SPARSE;
     return (1.2 * t_dense < t_sparse) ? HH_PREEXP_DENSE : HH_PREEXP_SPARSE;
 }
@@ -2960,8 +2959,10 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
             const char* bf = getenv("HH_GEMM_BLK_FMT");
             const int f16 = (mc->prune >= 6.2e-5f && !(bf && !strcmp(bf, "bf16"))) ? 1 : 0;
             if (mc->n_win > 0 && mc->d_blk_items && mc->col_lo == 0 && mc->col_hi == mc->n) {
-                const double est_sparse = (double)mc->cur_nnz * (double)mc->cur_nnz / (double)mc->n / 0.6e12;
-                const double est_gemm = mc->blk_flops * (f16 ? 4.0 / 6.0 : 1.0) / 1.2e15 + 2.0e-3;      // blk_flops counts six passes
+                // rates measured on one H100 SXM (400 W): Gustavson products 0.25e12/s (pre-expansion, C2 / C3), hh_k_syrk
+                // 2.9e14 issued flop/s (pre-expansion, C3)
+                const double est_sparse = (double)mc->cur_nnz * (double)mc->cur_nnz / (double)mc->n / 0.25e12;
+                const double est_gemm = mc->blk_flops * (f16 ? 4.0 / 6.0 : 1.0) / 2.9e14 + 2.0e-3;      // blk_flops counts six passes
                 blk = est_gemm < est_sparse;
             }
             if (blk) {
@@ -2987,7 +2988,7 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
                 hh_gemm_operand B = {d_blkB, np_op, mc->n, (int)mc->blk_ldk, mc->blk_ldk, (long long)plane, fmt};
                 HH_CHECK(hh_gemm_run(ctx, A, B, mc->d_blk_items, (int)mc->blk_items->size(), npass, pa, pb,
                                      env_int("HH_GEMM_CHUNK", f16 ? 2 : 1), d_blk_out, mc->blk_ldk, 0, mc->n, nullptr, nullptr,
-                                     hh_gemm_blk_out_scale(f16), 0, 0));
+                                     hh_gemm_blk_out_scale(f16), 0));
                 a.dense_in = d_blk_out;
                 a.ld = mc->blk_ldk;
                 mc->blk_iters++;

@@ -483,7 +483,7 @@ def bench_multi(a, world: int, rank_id: int, local: int):
                        "(all-to-all), disjoint partition tables all-gathered; MCL: pre-expansion and iteration 0 of every inflation on "
                        "column blocks x{0}, one all-gather of pruned columns per inflation, then inflation k runs on rank k mod {0} "
                        "alone".format(world),
-                       "cache": "inputs and the dense pre-expanded matrix exceed the 126 MB L2",
+                       "cache": "inputs and the dense pre-expanded matrix exceed the 50 MB L2",
                        "step": "route + all-to-all + link build + partition all-gather + index + CSC + normalise + pre-expansion + "
                                "MCL sweep"},
             "stage_ms": {"link_build_and_matrix": build_ms, "mcl_sweep": mcl_ms},

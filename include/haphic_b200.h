@@ -1,5 +1,5 @@
 /*
- * haphic_b200 -- C ABI of the B200-native `haphic cluster` hot path.
+ * haphic_b200 -- C ABI of the GPU-native (H100, sm_90a) `haphic cluster` hot path.
  *
  * This is the drop-in boundary: a plain C interface (pointers + sizes, no torch / C++ types)
  * that a maintainer of zengxiaofei/HapHiC would bind with ctypes from
@@ -178,7 +178,7 @@ int hh_mcl_create(hh_matrix* m, int expansion, int32_t col_lo, int32_t col_hi, h
 /* The same with the engine of the pre-expansion (2146-2149) chosen by the caller:
  *   HH_PREEXP_SPARSE  Gustavson SpGEMM on a shared-memory column accumulator (the reference's sparse mode,
  *                     mkl_matrix_power 2017-2023);
- *   HH_PREEXP_DENSE   the product as a symmetric dense GEMM on the tensor cores (tcgen05 / TMEM / TMA; 16-bit operand
+ *   HH_PREEXP_DENSE   the product as a symmetric dense GEMM on the tensor cores (wgmma / TMA; 16-bit operand
  *                     planes that reproduce the fp32 product to 2^-23, fp32 accumulation) -- the reference's dense mode
  *                     (`--dense_matrix`, numpy.linalg.matrix_power 2035 / 2149);
  *   HH_PREEXP_AUTO    whichever is estimated cheaper for this matrix (hh_mcl_create; env HH_MCL_PREEXP overrides).
@@ -189,9 +189,9 @@ typedef struct {
     int32_t mode;          /* HH_PREEXP_SPARSE or HH_PREEXP_DENSE: what ran                              */
     int32_t a_planes;      /* dense: 16-bit planes of the count operand (1: integer counts, 3: weights)    */
     int32_t passes;        /* dense: tensor-core passes per k-block                                        */
-    int32_t cta_group;     /* dense: 2 = CTA pairs (256 x 256 tiles), 1 = single CTAs (128 x 128)          */
+    int32_t cta_group;     /* dense: 1 = one CTA per 128 x 128 tile                                          */
     int32_t stages;        /* dense: shared-memory pipeline stages                                         */
-    int32_t chunk_kb;      /* dense: 64-wide k-blocks accumulated in TMEM between two register drains      */
+    int32_t chunk_kb;      /* dense: 64-wide k-blocks accumulated by wgmma between two round-to-nearest adds */
     float total_ms;        /* device time of the pre-expansion                                             */
     float densify_ms;      /* dense: operand planes from the CSC                                           */
     float gemm_ms;         /* dense: the GEMM kernel                                                       */

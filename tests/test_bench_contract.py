@@ -1,5 +1,6 @@
 """bench.py's JSON contract on the CPU side: the reference arm (`--impl reference`) runs here without a GPU and
-must print ONE line with the keys the driver reads."""
+must print ONE line with the keys a consumer of the benchmark reads.  It times the unmodified upstream reference, which
+is not part of this repository: build() installs it into oracle/_ref/ from a HapHiC checkout (see oracle/refimpl.py)."""
 
 import json
 import os
@@ -17,6 +18,7 @@ def test_reference_arm_line():
     lines = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]
     assert len(lines) == 1
     d = json.loads(lines[0])
+    assert "unavailable" not in d, d["unavailable"]
     assert d["impl"] == "reference" and d["metric"] == "hic_pairs_per_sec_matrix_build" and d["unit"] == "pairs/s"
     assert d["n_gpus"] == 1 and d["steps"] == 1 and d["warmup"] == 1 and d["higher_is_better"] is True
     assert d["value"] > 0 and d["ms_per_step"] > 0 and d["data"] == "synthetic" and d["vs_baseline"] is None
