@@ -39,6 +39,11 @@ class PreexpInfo(C.Structure):
                 ("clip", C.c_float), ("b_planes", C.c_int32), ("fmt_a", C.c_int32), ("fmt_b", C.c_int32), ("k_chunks", C.c_int32)]
 
 
+class CorrectRoundInfo(C.Structure):
+    _fields_ = [("n_examined", C.c_int32), ("n_broken", C.c_int32), ("n_breaks", C.c_int32), ("n_frag", C.c_int32),
+                ("n_links", C.c_int64)]
+
+
 HH_PREEXP_AUTO, HH_PREEXP_SPARSE, HH_PREEXP_DENSE = 0, 1, 2
 
 # name -> (restype, argtypes): every symbol include/haphic_b200.h declares
@@ -92,6 +97,15 @@ _SIGNATURES = {
     "hh_mcl_commit": (C.c_int, [_P]),
     "hh_mcl_set_block": (C.c_int, [_P, C.c_int32, C.c_int32]),
     "hh_mcl_destroy": (C.c_int, [_P]),
+    "hh_correct_create": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.POINTER(_P)]),
+    "hh_correct_add": (C.c_int, [_P, _P, C.c_int64, C.c_int]),
+    "hh_correct_round": (C.c_int, [_P, C.c_double, C.c_double, C.c_int64, C.c_int, C.POINTER(CorrectRoundInfo)]),
+    "hh_correct_fetch_breaks": (C.c_int, [_P, _P, _P, _P]),
+    "hh_correct_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hh_correct_fetch_cov": (C.c_int, [_P, _P, _P, _P]),
+    "hh_correct_set_layout": (C.c_int, [_P, _P, _P, _P, C.c_int32]),
+    "hh_correct_remap": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int]),
+    "hh_correct_destroy": (C.c_int, [_P]),
     "hh_pairs_open": (C.c_int, [C.c_char_p, _P, C.c_int32, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
     "hh_pairs_next": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "hh_pairs_close": (C.c_int, [_P]),

@@ -10,8 +10,10 @@ unchanged.  The per-read-pair link counting, dict_to_matrix and the Markov-clust
 libhaphic_b200.so on the GPU; file parsing, fragment statistics, filters on per-fragment scalars,
 result interpretation and the writers are host Python, as in the reference.
 
-Not supported (raise, never silently degrade): ``--correct_nrounds``, ``--ul``, ``--gfa`` (out of the hot-path scope,
-SURVEY.md section 2).
+Assembly correction (``--correct_nrounds``) runs on the GPU (haphic_b200/correct.py); the alignments are read once.
+
+Not supported (raise, never silently degrade): ``--ul`` (ignored with a warning together with ``--correct_nrounds``, as
+in the reference), ``--gfa`` (out of the hot-path scope, SURVEY.md section 2).
 
 Reference line numbers below refer to scripts/HapHiC_cluster.py (v1.0.7).
 """
@@ -1270,7 +1272,10 @@ def run(args, log_file=None):
                     "the iterates are stored sparsely in either mode")
     if args.aln_format == "auto":
         detect_format(args)
-    unsupported = [("--correct_nrounds", args.correct_nrounds), ("--ul", args.ul), ("--gfa", args.gfa)]
+    if args.correct_nrounds and args.ul:                   # 2774-2776
+        args.ul = None
+        logger.warning("Ultra-long data are not supported now when assembly correction is enabled")
+    unsupported = [("--ul", args.ul), ("--gfa", args.gfa)]
     for flag, val in unsupported:
         if val:
             raise NotImplementedError("haphic_b200: {} is not supported (out of the hot-path scope)".format(flag))
@@ -1285,16 +1290,26 @@ def run(args, log_file=None):
     read_depth_dict = dict()
     whitelist = set()
     args.whitelist = whitelist
+    from . import hicio
+
+    def open_alignments(inter_only):
+        name_index = hicio.NameIndex(list(fa_dict.keys()))
+        if args.aln_format == "bam":
+            return hicio.bam_batches(args.alignments, name_index, inter_only=inter_only, logger=logger, threads=args.threads)
+        return hicio.pairs_batches(args.alignments, args.aln_format, name_index, inter_only=inter_only, threads=args.threads)
+
+    alignments = None
+    if args.correct_nrounds:
+        # assembly correction (2798-2808) before stat_fragments: the one read of the alignments (all read1 records) feeds
+        # the coverage pass, and its batches -- remapped to the corrected contigs -- feed the link counting (2835-2851)
+        from . import correct
+        alignments, _nbroken = correct.run_correction(_context(), fa_dict, args, open_alignments(False),
+                                                      lambda seq: count_RE_sites(seq, args.RE))
     _, bin_set, bin_size, frag_len_dict, Nx_frag_set, RE_site_dict, split_ctg_set = stat_fragments(
         fa_dict, args.RE, read_depth_dict, whitelist, nchrs=args.nchrs, flank=args.flank, Nx=args.Nx, bin_size=args.bin_size)
-    from . import hicio
+    if alignments is None:
+        alignments = open_alignments(not split_ctg_set)     # bins need the intra-contig pairs too (2849-2856)
     names = list(fa_dict.keys())
-    name_index = hicio.NameIndex(names)
-    inter_only = not split_ctg_set          # bins need the intra-contig pairs too (2849-2856)
-    if args.aln_format == "bam":
-        alignments = hicio.bam_batches(args.alignments, name_index, inter_only=inter_only, logger=logger, threads=args.threads)
-    else:
-        alignments = hicio.pairs_batches(args.alignments, args.aln_format, name_index, inter_only=inter_only, threads=args.threads)
 
     # Two ways through the host side.  With --remove_allelic_links / --remove_concentrated_links the link dicts are
     # edited on the host, so they are built as the reference's Python objects.  Otherwise nothing on the host needs

@@ -185,3 +185,82 @@ def write_pairs(asm: Assembly, pairs: np.ndarray, path: str) -> None:
         f.write("## pairs format v1.0\n#columns: readID chr1 pos1 chr2 pos2 strand1 strand2\n")
         for r, (a, pa, b, pb) in enumerate(pairs.tolist()):
             f.write("r{}\t{}\t{}\t{}\t{}\t+\t-\n".format(r, names[a], pa + 1, names[b], pb + 1))
+
+
+def make_chimeras(asm: Assembly, pairs: np.ndarray, joins, span: int = 0, seed: int = 12345, window: int = 2000,
+                  gap: int = 0):
+    """Misjoined assemblies for assembly correction (``--correct_nrounds``): every tuple of contig ids in ``joins`` is
+    joined left to right into one contig named ``chimera{k}``; the joined contigs leave the FASTA and the chimeras follow
+    the remaining contigs.  ``pairs`` (int [P, 4]) is mapped onto the new contigs.
+
+    A junction bin always holds the ends of both joined contigs, so their own intra-contig pairs cover it: a plain junction
+    is a shallow valley, not an empty one.  ``gap`` > 0 drops every same-chimera record whose span [lo, hi] meets
+    [junction - gap, junction + gap) -- the bins inside that window get coverage 0 (a zero-coverage valley; with
+    gap >= 2 * resolution at least three bins).  ``span`` > 0 then appends, per junction, that many records with one end in
+    the ``window`` bp before the junction and one after it (a valley with non-zero coverage).
+    Returns (assembly, pairs, junctions) with junctions = [(chimera id, junction position)]."""
+    rng = np.random.default_rng(seed)
+    joined = {c for j in joins for c in j}
+    keep = [c for c in range(asm.n) if c not in joined]
+    new_id = np.full(asm.n, -1, np.int64)
+    offset = np.zeros(asm.n, np.int64)
+    new_id[keep] = np.arange(len(keep))
+    names = [asm.names[c] for c in keep]
+    lengths = [int(asm.lengths[c]) for c in keep]
+    junctions = []
+    for k, group in enumerate(joins):
+        cid = len(names)
+        at = 0
+        for m, c in enumerate(group):
+            if m:
+                junctions.append((cid, at))
+            new_id[c] = cid
+            offset[c] = at
+            at += int(asm.lengths[c])
+        names.append("chimera{}".format(k + 1))
+        lengths.append(at)
+    p = np.asarray(pairs, np.int64)
+    out = np.stack([new_id[p[:, 0]], p[:, 1] + offset[p[:, 0]], new_id[p[:, 2]], p[:, 3] + offset[p[:, 2]]], axis=1)
+    if gap > 0 and junctions:
+        cand = np.nonzero((out[:, 0] == out[:, 2]) & (out[:, 0] >= len(keep)))[0]
+        lo = np.minimum(out[cand, 1], out[cand, 3])
+        hi = np.maximum(out[cand, 1], out[cand, 3])
+        drop = np.zeros(len(cand), bool)
+        for cid, pos in junctions:
+            drop |= (out[cand, 0] == cid) & (lo < pos + gap) & (hi >= pos - gap)
+        out = np.delete(out, cand[drop], axis=0)
+    extra = []
+    for cid, pos in junctions:
+        for _ in range(span):
+            extra.append((cid, pos - 1 - int(rng.integers(0, window)), cid, pos + int(rng.integers(0, window))))
+    if extra:
+        out = np.concatenate([out, np.asarray(extra, np.int64)])
+    n = len(names)
+    new = Assembly(names, np.asarray(lengths, np.int64), np.zeros(n, np.int32), np.zeros(n, np.int64), np.zeros(n, np.int8),
+                   asm.chrom_len, asm.nchr)
+    return new, out.astype(np.int32), junctions
+
+
+def chimera_case(nchr: int, n_contigs: int, mean_len: int, n_pairs: int, n_joins: int, span: int, seed: int, group: int = 2,
+                 device: str = "cpu", gap: int = 1000):
+    """A seeded misjoined assembly: ``n_joins`` chimeras of ``group`` contigs, each from another chromosome than the one
+    before it.  The first half has ``span`` planted spanning records per junction (non-zero valleys); in the second half
+    every junction is a zero-coverage gap of +- ``gap`` bp (make_chimeras).  Returns (assembly, pairs, junctions)."""
+    asm = make_assembly(nchr, n_contigs, mean_len, seed=seed)
+    pairs = make_pairs(asm, n_pairs, seed=seed + 1, device=device).cpu().numpy()
+    rng = np.random.default_rng(seed + 2)
+    per_chr = asm.n // nchr
+    picks = rng.permutation(per_chr)[:group * n_joins]
+    joins = [tuple(int(picks[group * k + m]) + per_chr * ((m * (1 + k % (nchr - 1))) % nchr) for m in range(group))
+             for k in range(n_joins)]
+    a1, p1, j1 = make_chimeras(asm, pairs, joins[:n_joins // 2], span=span, seed=seed + 3)
+    if n_joins // 2 == n_joins:
+        return a1, p1, j1
+    # the second half: zero-coverage junctions (ids refer to the first result's contigs, whose order is preserved)
+    ids = {nm: i for i, nm in enumerate(a1.names)}
+    joins2 = [tuple(ids[asm.names[c]] for c in j) for j in joins[n_joins // 2:]]
+    a2, p2, j2 = make_chimeras(a1, p1, joins2, span=0, seed=seed + 4, gap=gap)
+    moved = {i: a2.names.index(a1.names[i]) for i, _ in j1}
+    for k in range(len(joins2)):
+        a2.names[-(len(joins2) - k)] = "chimera{}".format(n_joins // 2 + k + 1)
+    return a2, p2, [(moved[c], pos) for c, pos in j1] + j2

@@ -246,6 +246,45 @@ int hh_mcl_commit(hh_mcl* mc);
 int hh_mcl_set_block(hh_mcl* mc, int32_t col_lo, int32_t col_hi);
 int hh_mcl_destroy(hh_mcl* mc);
 
+/* ---- assembly correction (--correct_nrounds): correct_assembly and its helpers, HapHiC_cluster.py:943-1536 -----------
+ * Contigs are the ids 0 .. n_ctg-1 of the input FASTA; `resolution` = --correct_resolution.  Fragments under examination
+ * start as all contigs; after a round that is not the last they are the pieces of the fragments broken in it, with ids
+ * n_frag, n_frag + 1, ... (n_frag as reported by that round) in breakpoint-list order, left to right.
+ *   hh_correct_create: coverage arrays of len//res + 1 int32 bins per contig (1307-1311 / 1370-1374).
+ *   hh_correct_add: the coverage pass over a batch of records {ctg_a, pos_a, ctg_b, pos_b} (parse_pairs_for_correction
+ *     1321-1342, parse_bam_for_correction 1380-1396): same-contig records of contigs in the FASTA add 1 to the bins
+ *     [lo//res, hi//res] (numpy slice semantics) and are kept as links; every other record is ignored.
+ *   hh_correct_round: detect_break_points (943-1014) on the fragments under examination; unless last_round, the coverage
+ *     and link updates of break_and_update_ctgs (1063-1113, 1151-1153, 1176-1178, 1192-1197).
+ *   hh_correct_fetch_breaks: the round's breakpoints (fragment id, bin, coverage), n_breaks entries in the order of the
+ *     fragments under examination, ascending bins (a breakpoint sits at bin * res on its fragment).
+ *   hh_correct_info / hh_correct_fetch_cov: fragments under examination and their coverage slices, concatenated in order
+ *     (frag[n_active], nbins[n_active], cov[active_bins]).
+ *   hh_correct_set_layout: the corrected contigs, decided on the host (final_break_pos_dict / final_break_frag_dict,
+ *     1116-1170, and the re-ordered fa_dict): source contig c owns the entries [src_base[c], src_base[c+1]) of
+ *     piece_start (ascending, 0 first) / piece_id (id in the corrected fa_dict); an unbroken contig has one entry.
+ *   hh_correct_remap: convert_ctg of the *_for_correction generators (1401-1536): an end on contig c goes to the piece
+ *     with the largest start <= pos, at pos - start; ids outside [0, n_ctg) are kept.  rec_in / rec_out in `mem`. */
+typedef struct hh_correct hh_correct;
+typedef struct {
+    int32_t n_examined;  /* fragments examined in this round                            */
+    int32_t n_broken;    /* len(ctg_break_point_dict) (1214)                            */
+    int32_t n_breaks;    /* breakpoints in all                                           */
+    int32_t n_frag;      /* fragment ids before the round: the pieces' ids start here    */
+    int64_t n_links;     /* same-contig records kept by the coverage pass                */
+} hh_correct_round_info;
+int hh_correct_create(hh_ctx* ctx, int32_t n_ctg, const int64_t* ctg_len, int64_t resolution, hh_correct** out);
+int hh_correct_add(hh_correct* cr, const int32_t* rec, int64_t n_rec, int mem);
+int hh_correct_round(hh_correct* cr, double median_cov_ratio, double region_len_ratio, int64_t min_region_cutoff,
+                     int last_round, hh_correct_round_info* info);
+int hh_correct_fetch_breaks(hh_correct* cr, int32_t* frag, int32_t* bin, int32_t* cov);
+int hh_correct_info(hh_correct* cr, int32_t* n_active, int64_t* active_bins, int64_t* n_links);
+int hh_correct_fetch_cov(hh_correct* cr, int32_t* frag, int32_t* nbins, int32_t* cov);
+int hh_correct_set_layout(hh_correct* cr, const int32_t* src_base, const int64_t* piece_start, const int32_t* piece_id,
+                          int32_t n_pieces);
+int hh_correct_remap(hh_correct* cr, const int32_t* rec_in, int32_t* rec_out, int64_t n_rec, int mem);
+int hh_correct_destroy(hh_correct* cr);
+
 /* ---- host-side I/O around the path (native, no CUDA) ------------------------------------------------
  * .pairs / .pairs.gz reader: pairs_generator / pairs_generator_inter_ctgs, HapHiC_cluster.py:1539-1583.  Skips blank
  * and '#' lines, takes `cols[1], int(cols[2])-1, cols[3], int(cols[4])-1`, writes the two BED lines per pair
