@@ -455,13 +455,12 @@ int hh_gemm_run(hh_ctx* ctx, const hh_gemm_operand& A, const hh_gemm_operand& B,
 }
 
 static const int HG_P1[3][2] = {{0, 0}, {0, 1}, {0, 2}};
-static const int HG_P2[5][2] = {{0, 0}, {0, 1}, {1, 0}, {0, 2}, {1, 1}};
 static const int HG_P3[6][2] = {{0, 0}, {0, 1}, {1, 0}, {0, 2}, {1, 1}, {2, 0}};
 
-// pass list for `na` planes of A against three planes of B: every product of relative size >= 2^-16 (na = 1: exact)
+// pass list for `na` (1 or 3) planes of A against three planes of B: every product of relative size >= 2^-16 (na = 1: exact)
 int hh_gemm_passes(int na, int* pa, int* pb) {
-    const int(*pl)[2] = na == 1 ? HG_P1 : (na == 2 ? HG_P2 : HG_P3);
-    const int np = na == 1 ? 3 : (na == 2 ? 5 : 6);
+    const int(*pl)[2] = na == 1 ? HG_P1 : HG_P3;
+    const int np = na == 1 ? 3 : 6;
     for (int p = 0; p < np; ++p) {
         pa[p] = pl[p][0];
         pb[p] = pl[p][1];
@@ -503,13 +502,9 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
         int enc = 2;                                             // 0 = exact bf16, 2 = scaled f16
         if (fmt_env && !strcmp(fmt_env, "bf16")) enc = 0;
         if (flags & (1 | 4)) enc = 0;
-        int na = (flags & 1) ? 3 : 1;
+        const int na = (flags & 1) ? 3 : 1;
         const int nb = enc ? 2 : 3;
-        float clip = (flags & 1) ? 3.0e38f : (enc == 2 ? 2048.f : 256.f);
-        if (hg_env_int("HH_GEMM_NA", 0) == 2 && !(flags & 1) && enc == 0) {      // experiment: two planes instead of clipping
-            na = 2;
-            clip = 3.0e38f;
-        }
+        const float clip = (flags & 1) ? 3.0e38f : (enc == 2 ? 2048.f : 256.f);
         const int fmt_a = enc == 2 ? HH_GEMM_F16 : HH_GEMM_BF16, fmt_b = enc ? HH_GEMM_F16 : HH_GEMM_BF16;
         // The K range is cut into equal chunks when the operand planes of the whole range would exceed ~16 GB (a fifth of an
         // 80 GB device; 150k contigs: 135 GB): planes of one chunk at a time, the epilogue of every chunk after the first adds to M1.  The cut depends on
@@ -534,8 +529,6 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
             pb[0] = 0;
             pb[1] = 1;
         }
-        const int np_env = hg_env_int("HH_GEMM_NPASS", 0);      // experiments only: fewer passes = lower precision
-        if (np_env >= 1 && np_env < npass) npass = np_env;
         // k-blocks accumulated by the tensor core between two drains into the round-to-nearest registers: the tensor core's
         // accumulate truncates, so the bias grows with the number of accumulations (4 MMAs per k-block and pass); on dense
         // inputs (every product of similar size) 64 truncating accumulations reach 2.5e-6 of relative error.  Three k-blocks
