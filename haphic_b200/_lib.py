@@ -39,6 +39,14 @@ class PreexpInfo(C.Structure):
                 ("clip", C.c_float), ("b_planes", C.c_int32), ("fmt_a", C.c_int32), ("fmt_b", C.c_int32), ("k_chunks", C.c_int32)]
 
 
+class MclStepInfo(C.Structure):
+    _fields_ = [("it", C.c_int32), ("iter0", C.c_int32), ("iter0_w", C.c_int32), ("blk", C.c_int32), ("blk_f16", C.c_int32),
+                ("blk_chunk", C.c_int32), ("blk_ldk", C.c_int64), ("n_win", C.c_int32), ("n_big", C.c_int32),
+                ("wmax", C.c_int32), ("small", C.c_int32), ("small_cols", C.c_int32), ("small_overflow", C.c_int32),
+                ("col", C.c_int32), ("col_cols", C.c_int32), ("col_w", C.c_int32), ("col_smem", C.c_int32),
+                ("col_track", C.c_int32), ("col_flat", C.c_int32)]
+
+
 class CorrectRoundInfo(C.Structure):
     _fields_ = [("n_examined", C.c_int32), ("n_broken", C.c_int32), ("n_breaks", C.c_int32), ("n_frag", C.c_int32),
                 ("n_links", C.c_int64)]
@@ -95,6 +103,7 @@ _SIGNATURES = {
     "hh_mcl_pack": (C.c_int, [_P, _P, _P, _P]),
     "hh_mcl_unpack": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int64]),
     "hh_mcl_commit": (C.c_int, [_P]),
+    "hh_mcl_step_info": (C.c_int, [_P, C.POINTER(MclStepInfo)]),
     "hh_mcl_set_block": (C.c_int, [_P, C.c_int32, C.c_int32]),
     "hh_mcl_destroy": (C.c_int, [_P]),
     "hh_correct_create": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.POINTER(_P)]),

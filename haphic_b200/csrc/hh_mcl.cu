@@ -1519,6 +1519,7 @@ struct hh_mcl {
     int preexp_mode;               // HH_PREEXP_SPARSE or HH_PREEXP_DENSE: the engine that built M1
     float clip_ms;                 // dense engine: the sparse correction for counts above HH_CLIP
     hh_gemm_stats gemm;            // tensor-core path: planes, passes, flops, times
+    hh_mcl_step_info_t info;       // engines of the last hh_mcl_step (hh_mcl_step_info)
 };
 
 static void slot_free(hh_slotmat& s) {
@@ -2355,8 +2356,10 @@ extern "C" int hh_mcl_create_ex(hh_matrix* m, int expansion, int32_t col_lo, int
     mc->own_hi = col_hi;
     mc->expansion = expansion;
     mc->cur = -1;
-    // higher powers go through the plain column kernel: A . (A . (... A)), one factor at a time
+    // higher powers go through the plain column kernel: A . (A . (... A)), one factor at a time.  0 = never, 1 = when the
+    // cost model prefers it, 2 = on every step where it is possible (tests)
     mc->use_blk = (expansion == 2) ? env_int("HH_MCL_BLOCKGEMM", 1) : 0;
+    mc->info.it = -1;
     mc->blk_items = new std::vector<hh_gemm_item>();
     const hh_geom g = geom_for(ctx, m->n);
     mc->W = g.W;
@@ -2624,7 +2627,10 @@ static int mcl_build_perm(hh_mcl* mc) {
         HH_LAUNCH(ctx, hh_k_cc_init, (n + 255) / 256, 256, 0, d_lab, n);
         int grid = (n + 7) / 8;
         if (grid > ctx->sm_count * 16) grid = ctx->sm_count * 16;
-        for (int round = 0; round < 64; ++round) {
+        // until no label changes: the windows below are only valid for converged labels.  A round moves the smallest
+        // label at least one hop, so a long chain-like component (a ring of contigs) can need hundreds of rounds.
+        for (int round = 0;; ++round) {
+            HH_REQUIRE(round <= n, HH_ERR_STATE, "hh_mcl: component labels did not converge");
             HH_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), ctx->stream));
             HH_LAUNCH(ctx, hh_k_cc_hook, grid, 256, 0, M, d_lab, d_flag);
             HH_LAUNCH(ctx, hh_k_cc_jump, (n + 255) / 256, 256, 0, d_lab, n);
@@ -2735,6 +2741,8 @@ extern "C" int hh_mcl_begin(hh_mcl* mc, double inflation, double pruning) {
     mc->col_lo = mc->own_lo;      // hh_mcl_set_block is per mcl() call
     mc->col_hi = mc->own_hi;
     mc->begun = true;
+    memset(&mc->info, 0, sizeof(mc->info));
+    mc->info.it = -1;
     return HH_OK;
 }
 
@@ -2757,10 +2765,27 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
     a.out = mc->it[dst];
     HH_CUDA(cudaEventRecord(mc->ev0, ctx->stream));
     const int ncols_owned = mc->col_hi - mc->col_lo;
+    hh_mcl_step_info_t& info = mc->info;
+    memset(&info, 0, sizeof(info));
+    info.it = -1;
+    info.n_win = mc->n_win;
+    info.n_big = mc->n_big;
+    info.wmax = mc->wmax;
+    auto note_col = [&](int ncols) {
+        info.col = 1;
+        info.col_cols = ncols;
+        info.col_w = g.W;
+        info.col_smem = g.smem_acc ? 1 : 0;
+        info.col_track = a.track;
+        info.col_flat = a.flat;
+    };
+    bool small_ran = false;
     if (it == 0) {
         a.dense_in = mc->d_m1;
         a.do_conv = 0;
         HH_CHECK(launch_iter0(ctx, g, a));
+        info.iter0 = 1;
+        info.iter0_w = g.W;
     } else if (mc->perm_space) {
         a.A = mc->it[mc->cur];
         a.B = mc->it[mc->cur];
@@ -2780,6 +2805,9 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
             a.order = mc->d_overflow;
             a.ncols_ptr = mc->d_bigcount;
             HH_CHECK((launch_col<SRC_PRODUCT, EPI_PRUNE>(ctx, g, mc->d_scratch, mc->grid_cap, a)));
+            // size of the overflow list, read with the step's statistics below
+            HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 24, mc->d_bigcount, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            small_ran = true;
         } else {
             // Window components whose block product is cheaper as a GEMM: both operands as three exact bf16 planes (six
             // passes), drained every k-block; the expansion of hh_k_col_win is replaced, its epilogue is not.
@@ -2795,7 +2823,7 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
                 // 2.9e14 issued flop/s (pre-expansion, C3)
                 const double est_sparse = (double)mc->cur_nnz * (double)mc->cur_nnz / (double)mc->n / 0.25e12;
                 const double est_gemm = mc->blk_flops * (f16 ? 4.0 / 6.0 : 1.0) / 2.9e14 + 2.0e-3;      // blk_flops counts six passes
-                blk = est_gemm < est_sparse;
+                blk = mc->use_blk == 2 || est_gemm < est_sparse;
             }
             if (blk) {
                 const int np_op = f16 ? 2 : 3;
@@ -2818,12 +2846,17 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
                 const int fmt = f16 ? HH_GEMM_F16 : HH_GEMM_BF16;
                 hh_gemm_operand A = {d_blkA, np_op, mc->n, (int)mc->blk_ldk, mc->blk_ldk, (long long)plane, fmt};
                 hh_gemm_operand B = {d_blkB, np_op, mc->n, (int)mc->blk_ldk, mc->blk_ldk, (long long)plane, fmt};
+                const int chunk = env_int("HH_GEMM_CHUNK", f16 ? 2 : 1);
                 HH_CHECK(hh_gemm_run(ctx, A, B, mc->d_blk_items, (int)mc->blk_items->size(), npass, pa, pb,
-                                     env_int("HH_GEMM_CHUNK", f16 ? 2 : 1), d_blk_out, mc->blk_ldk, 0, mc->n, nullptr, nullptr,
+                                     chunk, d_blk_out, mc->blk_ldk, 0, mc->n, nullptr, nullptr,
                                      hh_gemm_blk_out_scale(f16), 0));
                 a.dense_in = d_blk_out;
                 a.ld = mc->blk_ldk;
                 mc->blk_iters++;
+                info.blk = 1;
+                info.blk_f16 = f16;
+                info.blk_chunk = chunk;
+                info.blk_ldk = mc->blk_ldk;
             }
             if (mc->n_win > 0) {
                 const size_t smem = (size_t)mc->wmax * sizeof(float);
@@ -2848,6 +2881,7 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
                 a.order = mc->d_big_list;
                 a.ncols = mc->n_big;
                 HH_CHECK((launch_col<SRC_PRODUCT, EPI_PRUNE>(ctx, g, mc->d_scratch, mc->grid_cap, a)));
+                note_col(mc->n_big);
             }
         }
     } else {
@@ -2868,10 +2902,19 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
         a.track = (dcol * dcol * 4.0 < (double)mc->n) ? 1 : 0;
         a.flat = choose_flat(mc, (double)mc->cur_nnz);
         HH_CHECK((launch_col<SRC_PRODUCT, EPI_PRUNE>(ctx, g, mc->d_scratch, mc->grid_cap, a)));
+        note_col(ncols_owned);
     }
     HH_CUDA(cudaEventRecord(mc->ev1, ctx->stream));
     unsigned long long st[4];
     HH_CHECK(read_stats(ctx, mc->d_stats, st));
+    if (small_ran) {
+        const int overflow = *reinterpret_cast<const int*>(ctx->h_scratch + 24);
+        info.small = 1;
+        info.small_overflow = overflow;
+        info.small_cols = ncols_owned - overflow;
+        if (overflow > 0) note_col(overflow);
+    }
+    info.it = it;
     if (kernel_ms) HH_CUDA(cudaEventElapsedTime(kernel_ms, mc->ev0, mc->ev1));
     HH_REQUIRE((int)(st[3] & 0xffffffffull) == 0, HH_ERR_CAPACITY,
                "hh_mcl_step: a pruned column exceeded its slot (%d entries); pruning threshold too small for this layout", mc->it_cap);
@@ -2887,6 +2930,12 @@ extern "C" int hh_mcl_step(hh_mcl* mc, int it, int64_t* nnz_owned, int64_t* prod
     mc->pending = dst;
     mc->have_pending = true;
     mc->last_step_it = it;
+    return HH_OK;
+}
+
+extern "C" int hh_mcl_step_info(hh_mcl* mc, hh_mcl_step_info_t* info) {
+    HH_REQUIRE(mc && info, HH_ERR_ARG, "hh_mcl_step_info: NULL argument");
+    *info = mc->info;
     return HH_OK;
 }
 

@@ -11,7 +11,7 @@ from decimal import Decimal
 
 import numpy as np
 
-from ._lib import HH_PREEXP_AUTO, HH_PREEXP_DENSE, HH_PREEXP_SPARSE, MclResult, PreexpInfo, check, load, ptr
+from ._lib import HH_PREEXP_AUTO, HH_PREEXP_DENSE, HH_PREEXP_SPARSE, MclResult, MclStepInfo, PreexpInfo, check, load, ptr
 from .links import LinkMatrix
 
 
@@ -102,6 +102,12 @@ class Mcl:
         check(load().hh_mcl_step(self._h, int(it), C.byref(nnz), C.byref(prod), C.byref(delta), C.byref(ms)))
         self.last_step_ms = float(ms.value)
         return int(nnz.value), int(prod.value), float(delta.value)
+
+    def step_info(self) -> dict:
+        """Engines the last step ran (hh_mcl_step_info): iteration 0 stream, block GEMM, window / small / column kernels."""
+        si = MclStepInfo()
+        check(load().hh_mcl_step_info(self._h, C.byref(si)))
+        return {k: getattr(si, k) for k, _t in MclStepInfo._fields_}
 
     def pack(self, nnz_owned: int):
         """Owned block of the pending iterate as CUDA tensors (len int32 [ncols], idx int32, val fp32)."""

@@ -240,6 +240,30 @@ int hh_mcl_pack(hh_mcl* mc, int32_t* len_dev, int32_t* idx_dev, float* val_dev);
 int hh_mcl_unpack(hh_mcl* mc, int32_t col_lo, int32_t col_hi, const int32_t* len_dev,
                   const int32_t* idx_dev, const float* val_dev, int64_t nnz_block);
 int hh_mcl_commit(hh_mcl* mc);
+/* which engines the last hh_mcl_step ran (tests assert with it that the path they target was taken).  Counts are of the
+ * columns this context computed in that step. */
+typedef struct {
+    int32_t it;              /* iteration number of the step (-1: no step since hh_mcl_begin)                      */
+    int32_t iter0;           /* 1: hh_k_iter0 streamed the dense M1                                              */
+    int32_t iter0_w;         /* its W (row blocks per column)                                                    */
+    int32_t blk;             /* 1: the window components were multiplied by the block GEMM on the tensor cores   */
+    int32_t blk_f16;         /* block GEMM operands: 1 = two f16 planes of M * 2^14 (four passes), 0 = three bf16 */
+    int32_t blk_chunk;       /* block GEMM: k-blocks accumulated by wgmma between two round-to-nearest adds      */
+    int64_t blk_ldk;         /* block GEMM: row pitch of the operand planes (largest window component, padded)   */
+    int32_t n_win;           /* columns of window components (hh_k_col_win, or the block GEMM's epilogue)       */
+    int32_t n_big;           /* columns of components wider than the window                                      */
+    int32_t wmax;            /* window accumulator size                                                          */
+    int32_t small;           /* 1: the nearly-converged branch ran hh_k_col_small                                */
+    int32_t small_cols;      /* columns hh_k_col_small finished                                                  */
+    int32_t small_overflow;  /* columns it sent to its overflow list (finished by hh_k_col)                      */
+    int32_t col;             /* 1: hh_k_col<product, prune> was launched                                         */
+    int32_t col_cols;        /* columns it was given (the overflow list, the wide components, or all owned)      */
+    int32_t col_w;           /* its W                                                                            */
+    int32_t col_smem;        /* 1: shared-memory accumulator, 0: global                                          */
+    int32_t col_track;       /* TRACK (dirty-chunk bitmap)                                                       */
+    int32_t col_flat;        /* FLAT (flat 32-entry walk)                                                        */
+} hh_mcl_step_info_t;
+int hh_mcl_step_info(hh_mcl* mc, hh_mcl_step_info_t* info);
 /* change the block of columns the following steps compute (between hh_mcl_commit and hh_mcl_step, after iteration 0;
  * reset by hh_mcl_begin).  Column shards switch to (0, n) once the iterate is tiny: no exchange is needed any more
  * because every rank then computes the identical full iterate. */
