@@ -83,6 +83,8 @@ _SIGNATURES = {
     "hh_links_destroy": (C.c_int, [_P]),
     "hh_links_linked_index": (C.c_int, [_P, _P, _P, C.POINTER(C.c_int32)]),
     "hh_matrix_from_links": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int, C.c_int, C.POINTER(_P)]),
+    "hh_links_linked_index_phased": (C.c_int, [_P, _P, C.c_int, _P, C.c_double, _P, C.POINTER(C.c_int32)]),
+    "hh_matrix_from_links_phased": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int, C.c_int, _P, C.c_double, C.POINTER(_P)]),
     "hh_matrix_rank_sums": (C.c_int, [_P, C.c_int, _P]),
     "hh_matrix_from_csc": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "hh_matrix_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
@@ -124,6 +126,7 @@ _SIGNATURES = {
     "hh_bam_next": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "hh_bam_close": (C.c_int, [_P]),
     "hh_pickle_links": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P]),
+    "hh_pickle_links_mixed": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, _P, C.c_int64, _P, _P]),
     "hh_clm_from_records": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, C.c_int64, _P, _P, C.c_int]),
 }
 

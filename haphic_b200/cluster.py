@@ -12,8 +12,13 @@ result interpretation and the writers are host Python, as in the reference.
 
 Assembly correction (``--correct_nrounds``) runs on the GPU (haphic_b200/correct.py); the alignments are read once.
 
+``--gfa`` (hifiasm GFA files, one per haplotype) reads the read depths and haplotypes (parse_gfa): the read-depth filter runs
+in filter_fragments on the host, and with two or more files the inter-haplotype reduction of the flank links
+(reduce_inter_hap_HiC_links) runs inside the device matrix kernels; the contig-level full links are reduced on the fetched
+arrays.  ``--phasing_weight`` must lie in [0, 1].
+
 Not supported (raise, never silently degrade): ``--ul`` (ignored with a warning together with ``--correct_nrounds``, as
-in the reference), ``--gfa`` (out of the hot-path scope, SURVEY.md section 2).
+in the reference).
 
 Reference line numbers below refer to scripts/HapHiC_cluster.py (v1.0.7).
 """
@@ -102,7 +107,69 @@ def determine_int_type(fa_dict, logger=logger):
 
 
 def parse_gfa(gfa_list, fa_dict, logger=logger):
-    raise NotImplementedError("haphic_b200: --gfa (hifiasm read depth / phasing, HapHiC_cluster.py:150-185) is not supported")
+    """{ctg: (index of the GFA file in gfa_list, read depth)} from the `S` lines of hifiasm GFA files (150-185): LN:i: is
+    checked against the FASTA, rd:i: is the read depth, and a contig named in several files keeps the last one.  Every
+    FASTA contig must be in some file.  `haphic reassign --gfa` imports this name (HapHiC_reassign.py:23)."""
+    logger.info("Parsing input gfa file(s)...")
+    read_depth_dict = dict()
+    for hap, gfa in enumerate(gfa_list):
+        with open(gfa) as f:
+            for line in f:
+                if not line.startswith("S\t"):
+                    continue
+                # at most six fields: the sequence column (index 2) can be megabases long and is never needed
+                cols = line.split("\t", 5)
+                ctg = cols[1]
+                length = int(cols[3].split(":")[-1])
+                depth = int(cols[4].split(":")[-1])
+                if ctg in fa_dict and length != fa_dict[ctg][1]:
+                    logger.error("The contig {} in gfa file {} has a different length than the one in the fasta file. "
+                                 "Maybe the gfa file does not match the fasta file.".format(ctg, gfa))
+                    raise RuntimeError("The contig {} in gfa file {} has a different length than the one in the fasta file. "
+                                       "Maybe the gfa file(s) does not match the fasta file.".format(ctg, gfa))
+                read_depth_dict[ctg] = (hap, depth)
+    for ctg in fa_dict:
+        if ctg not in read_depth_dict:
+            msg = "Can not find contig {} in the gfa file(s). Maybe the gfa file(s) does not match the fasta file.".format(ctg)
+            logger.error(msg)
+            raise RuntimeError(msg)
+    if len(read_depth_dict) > len(fa_dict):
+        logger.warning("The number of contigs in the gfa file(s) ({}) is greater than that in the fasta file ({}). "
+                       "Maybe some contigs were removed in the fasta file?".format(len(read_depth_dict), len(fa_dict)))
+    return read_depth_dict
+
+
+def haplotype_array(read_depth_dict, names):
+    """int32 haplotype index (GFA file index of parse_gfa) of every name."""
+    return np.fromiter((read_depth_dict[n][0] for n in names), dtype=np.int32, count=len(names))
+
+
+def reduce_inter_hap_HiC_links(link_dict, read_depth_dict, phasing_weight, target="flank_link_dict", names=None):
+    """695-707: every link between two different haplotypes becomes ``v - v * phasing_weight`` (two roundings) and is
+    deleted when that is 0; the other entries keep their order and type.
+
+    ``link_dict`` is the reference's dict (edited in place), a LinkArrays (fp64 pass on the arrays, LinkArrays.reduce_phasing)
+    or the device LinkTable with its fragment ``names``: the flank links then stay on the device and the reduction runs
+    inside the matrix kernels (hh_matrix_from_links_phased), so this only returns the haplotype array of the table's
+    fragments for device_matrix."""
+    logger.info("Reducing inter-haplotype Hi-C links in {}...".format(target))
+    from .links import LinkTable
+    if isinstance(link_dict, LinkTable):
+        return haplotype_array(read_depth_dict, names)
+    if isinstance(link_dict, LinkArrays):
+        link_dict.reduce_phasing(haplotype_array(read_depth_dict, link_dict.names), phasing_weight)
+        return None
+    deleted = []
+    for pair, links in link_dict.items():
+        if read_depth_dict[pair[0]][0] == read_depth_dict[pair[1]][0]:
+            continue
+        links = links - links * phasing_weight
+        link_dict[pair] = links
+        if links == 0:
+            deleted.append(pair)
+    for pair in deleted:
+        del link_dict[pair]
+    return None
 
 
 def remove_allelic_HiC_links(fa_dict, ctg_coord_dict, full_link_dict, args, flank_link_dict=None, filtered_frags=None,
@@ -497,18 +564,21 @@ def _cut_index(sorted_pairs, limit, inclusive):
     return len(sorted_pairs)
 
 
-def device_matrix(table, names, frag_set, normalize_by_nlinks=False, add_self_loops=True):
+def device_matrix(table, names, frag_set, normalize_by_nlinks=False, add_self_loops=True, hap=None, phasing_weight=0.0):
     """dict_to_matrix (310-373) on the device table: (LinkMatrix, frag_index_dict).  Linked fragments get their
-    first-seen index on the GPU; kept-but-unlinked ones follow in the reference's set-iteration order (355-359)."""
+    first-seen index on the GPU; kept-but-unlinked ones follow in the reference's set-iteration order (355-359).
+    ``hap`` (haplotype per table fragment) builds it from the phasing-reduced dict (reduce_inter_hap_HiC_links): a
+    fragment whose links were all deleted joins the unlinked tail."""
     keep = np.fromiter((n in frag_set for n in names), dtype=np.uint8, count=len(names))
-    index, n_linked = table.linked_index(keep)
+    index, n_linked = table.linked_index(keep, hap=hap, phasing_weight=phasing_weight, normalize_by_nlinks=normalize_by_nlinks)
     order = np.argsort(np.where(index >= 0, index, np.iinfo(np.int32).max), kind="stable")[:n_linked]
     frags_in_dict = set()
     for c in order.tolist():                    # same insertion order as 332-333
         frags_in_dict.add(names[c])
     ids = {n: i for i, n in enumerate(names)}
     tail = [ids[f] for f in frag_set - frags_in_dict]
-    matrix = table.to_matrix(keep, tail, normalize_by_nlinks=normalize_by_nlinks, add_self_loops=add_self_loops)
+    matrix = table.to_matrix(keep, tail, normalize_by_nlinks=normalize_by_nlinks, add_self_loops=add_self_loops, hap=hap,
+                             phasing_weight=phasing_weight)
     frag_index = {names[c]: int(index[c]) for c in order.tolist()}
     for k, c in enumerate(tail):
         frag_index[names[c]] = n_linked + k
@@ -521,8 +591,6 @@ def filter_fragments(Nx_frag_set, RE_site_dict, RE_site_cutoff, frag_link_dict, 
     """Same decisions and log lines as the reference's filter_fragments (741-940).  With ``device_table`` the
     O(n^2 log n) rank-sum part (864-892) runs on the GPU (hh_matrix_rank_sums); otherwise on the host."""
     logger.info("Filtering fragments...")
-    if read_depth_dict:
-        raise NotImplementedError("haphic_b200: read-depth filtering (--gfa) is not supported")
     wl_frags = set()
     density = []
     total_links, total_RE = 0, 1
@@ -567,7 +635,41 @@ def filter_fragments(Nx_frag_set, RE_site_dict, RE_site_cutoff, frag_link_dict, 
     logger.info("[link density filtering] {} fragments removed, {} fragments kept".format(remaining - len(filtered), len(filtered)))
     for frag, d in density[:lower] + density[upper:]:
         logger.debug("[link density filtering] Fragment {} is removed, density={}".format(frag, d))
+    unfiltered = density
     density = density[lower:upper]
+
+    # read-depth filtering (819-862, --gfa): an IQR outlier cut on the depths of all RE-filtered fragments, intersected with
+    # the density survivors.  `upper` still holds the density window's bound: with an empty depth list the "multiple" scan
+    # starts from it, like the reference's for/else
+    if read_depth_dict:
+        depths = sorted(((frag, read_depth_dict[frag][1]) for frag, _ in unfiltered), key=lambda x: x[1])
+        p_rd = check_param("--read_depth_upper", read_depth_upper, {"X", "x"})
+        q1, med, q3 = np.quantile([d for _, d in depths], (0.25, 0.5, 0.75))
+        iqr = q3 - q1
+        logger.info("[read depth filtering] Q1={}, median={}, Q3={}, IQR=Q3-Q1={}".format(q1, med, q3, iqr))
+        if p_rd[-1]:
+            limit = q3 + p_rd[0] * iqr
+            for upper, (_f, d) in enumerate(depths):
+                if d > limit:
+                    break
+            else:
+                upper += 1
+            logger.info('[read depth filtering] Parameter --read_depth_upper {} is set to "multiple" mode and equivalent to {} in "fraction" mode'.format(
+                read_depth_upper, upper / remaining))
+        else:
+            upper = int(remaining * float(read_depth_upper))
+            logger.info('[read depth filtering] Parameter --read_depth_upper {} is set to "fraction" mode and equivalent to {}X in "multiple" mode'.format(
+                read_depth_upper, (depths[max(0, upper - 1)][1] - q3) / iqr))
+        filtered = filtered & {frag for frag, _ in depths[:upper]}
+        # the removed count leaves out fragments the density window already dropped -- as the reference counts them, with the
+        # depth cut's position also slicing the density list
+        by_density = {frag for frag, _ in unfiltered[:lower] + unfiltered[upper:]}
+        by_depth_only = {frag for frag, _ in depths[upper:]} - by_density
+        logger.info("[read depth filtering] {} fragments removed, {} fragments kept".format(len(by_depth_only), len(filtered)))
+        for frag, d in depths[upper:]:
+            if frag in by_depth_only:
+                logger.debug("[read depth filtering] Fragment {} is removed, read depth={}".format(frag, d))
+        density = [(frag, d) for frag, d in density if frag in filtered]
 
     # rank-sum of the topN nearest fragments (864-927)
     if device_table is not None:
@@ -858,9 +960,32 @@ class LinkArrays:
         self.key_i = np.ascontiguousarray(key_i, dtype=np.int32)
         self.key_j = np.ascontiguousarray(key_j, dtype=np.int32)
         self.values = np.ascontiguousarray(values, dtype=np.int64)
+        # None: every value is a Python int (int64 values).  Else values are fp64 and is_float[e] says whether entry e is a
+        # Python float in the reference's dict (an inter-haplotype link reduced by a fractional phasing weight).
+        self.is_float = None
 
     def __len__(self):
         return len(self.key_i)
+
+    def reduce_phasing(self, hap, phasing_weight):
+        """reduce_inter_hap_HiC_links (695-707) on the arrays: entries between haplotypes (``hap`` per contig) become
+        v - v * w in fp64 (two roundings, as Python evaluates it), zeros are dropped, the order is kept.  With w = 1 every
+        such entry is dropped and the values stay integers."""
+        inter = hap[self.key_i] != hap[self.key_j]
+        if not inter.any():
+            return
+        x = self.values.astype(np.float64)
+        xi = x[inter]
+        x[inter] = xi - xi * float(phasing_weight)
+        keep = x != 0
+        self.key_i, self.key_j = self.key_i[keep], self.key_j[keep]
+        inter = inter[keep]
+        if self.is_float is None and not inter.any():
+            self.values = self.values[keep]
+        else:
+            self.is_float = inter if self.is_float is None else (self.is_float[keep] | inter)
+            self.values = x[keep]
+        self._directed = self._directed_dev = None
 
     def directed(self):
         """(L, ctg, other): the symmetric link matrix as CSR (int64 values) and the 2 * nnz directed entries interleaved in the
@@ -892,15 +1017,27 @@ class LinkArrays:
     def to_dict(self):
         d = defaultdict(int)
         names = self.names
-        for a, b, v in zip(self.key_i.tolist(), self.key_j.tolist(), self.values.tolist()):
+        for a, b, v in zip(self.key_i.tolist(), self.key_j.tolist(), self.python_values()):
             d[(names[a], names[b])] = v
         return d
+
+    def python_values(self):
+        """The values as the reference's dict holds them: ints, and floats where is_float."""
+        if self.is_float is None:
+            return self.values.tolist()
+        return [v if f else int(v) for v, f in zip(self.values.tolist(), self.is_float.tolist())]
 
     def write_pickle(self, path, ht=None):
         """full_links.pkl (or HT_links.pkl when the [n, 4] HT counters are given) with the native writer."""
         from . import hicio
         from ._lib import check, load, ptr
         n = len(self.key_i)
+        if self.is_float is not None and ht is None:
+            flags = np.ascontiguousarray(self.is_float, dtype=np.uint8)
+            check(load().hh_pickle_links_mixed(os.fsencode(path), hicio.names_blob(self.names), len(self.names),
+                                               ptr(self.key_i) if n else None, ptr(self.key_j) if n else None, n,
+                                               ptr(self.values) if n else None, ptr(flags) if n else None))
+            return
         check(load().hh_pickle_links(os.fsencode(path), hicio.names_blob(self.names), len(self.names), ptr(self.key_i) if n else None,
                                      ptr(self.key_j) if n else None, n, ptr(self.values) if ht is None else None, None,
                                      ptr(np.ascontiguousarray(ht, dtype=np.uint32)) if ht is not None else None))
@@ -918,17 +1055,27 @@ def ranked_group_links(link_dict, ctg_group_dict):
     return _ranked_lists(link_dict.names, *arr[1:])
 
 
+def _python_numbers(sums, is_float):
+    """Sums as the reference's dict values: ints, or floats where any contributing link was a float."""
+    if is_float is None:
+        return sums.tolist()
+    return [v if f else int(v) for v, f in zip(sums.tolist(), is_float.tolist())]
+
+
 def _ranked_group_arrays(link_dict, ctg_group_dict):
-    """(gid, contig, group, links) of the same ranking as flat arrays ordered by (contig, rank); None when nothing is linked to
-    a group.  gid[c] = group of contig c (-1 = ungrouped)."""
+    """(gid, contig, group, links, is_float) of the same ranking as flat arrays ordered by (contig, rank); None when nothing
+    is linked to a group.  gid[c] = group of contig c (-1 = ungrouped).  is_float is None for integer links; after a
+    fractional phasing weight (LinkArrays.is_float) links are fp64 sums and is_float marks the float-valued ones."""
     names = link_dict.names
     n = len(names)
     gid = np.array([-1 if ctg_group_dict[nm] == "ungrouped" else ctg_group_dict[nm] for nm in names], dtype=np.int64)
     if len(link_dict) == 0 or gid.max() < 0:
         return None
     ng = int(gid.max()) + 1
+    if link_dict.is_float is not None:
+        return (gid,) + _ranked_group_links_mixed(link_dict, gid, ng)
     if _CTX is not None and os.environ.get("HAPHIC_STATS_DEVICE", "1") != "0":
-        return (gid,) + tuple(_ranked_group_links_device(link_dict, gid, ng, _CTX.device))
+        return (gid,) + tuple(_ranked_group_links_device(link_dict, gid, ng, _CTX.device)) + (None,)
     # links of every contig into every group = (symmetric link matrix) x (contig -> group indicator): one sparse product per
     # inflation instead of a sort of all 2 * nnz directed entries (20 sorts of 1.2e8 keys took 15 min at 50k contigs)
     import scipy.sparse as sp
@@ -962,16 +1109,53 @@ def _ranked_group_arrays(link_dict, ctg_group_dict):
         mine = np.nonzero(tie[c_of])[0]
         first[mine] = tab[trow[c_of[mine]] * ng + g_of[mine]]
     rank = np.lexsort((first, -sums, c_of))
-    return gid, c_of[rank], g_of[rank], sums[rank]
+    return gid, c_of[rank], g_of[rank], sums[rank], None
 
 
-def _ranked_lists(names, c_of, g_of, sums):
+def _ranked_group_links_mixed(link_dict, gid, ng):
+    """The ranking for int / float links.  parse_link_dict (2245-2258) adds a contig's links to one group one by one in its
+    visiting order, starting from int 0: integer prefixes are exact in fp64, so plain sequential fp64 adds in that order give
+    its sums, and a sum is a float iff one of its links is.  The adds run position by position across all (contig, group)
+    segments at once, longest segments first, so every step works on a prefix of the segments."""
+    m = len(link_dict)
+    ctg = np.empty(2 * m, np.int64)
+    oth = np.empty(2 * m, np.int64)
+    ctg[0::2], ctg[1::2] = link_dict.key_i, link_dict.key_j
+    oth[0::2], oth[1::2] = link_dict.key_j, link_dict.key_i
+    g = gid[oth]
+    pos = np.nonzero(g >= 0)[0]                                 # position in the visiting order
+    if len(pos) == 0:
+        z = np.zeros(0, np.int64)
+        return z, z, np.zeros(0, np.float64), np.zeros(0, bool)
+    key = ctg[pos] * ng + g[pos]
+    order = np.argsort(key, kind="stable")                     # by key, then by position
+    ks = key[order]
+    val = np.repeat(link_dict.values, 2)[pos][order]
+    flt = np.repeat(link_dict.is_float, 2)[pos][order]
+    starts = np.concatenate([[0], np.nonzero(np.diff(ks))[0] + 1])
+    seg_len = np.diff(np.concatenate([starts, [len(ks)]]))
+    by_len = np.argsort(-seg_len, kind="stable")
+    st_sorted, len_sorted = starts[by_len], seg_len[by_len]
+    acc = np.zeros(len(starts), np.float64)
+    for p in range(int(len_sorted[0])):
+        k = int(np.searchsorted(-len_sorted, -p, side="left"))   # segments longer than p: a prefix
+        acc[:k] += val[st_sorted[:k] + p]
+    sums = np.empty(len(starts), np.float64)
+    sums[by_len] = acc
+    is_f = np.logical_or.reduceat(flt, starts)
+    first = pos[order][starts]                                  # first position of each segment
+    c_of, g_of = ks[starts] // ng, ks[starts] % ng
+    rank = np.lexsort((first, -sums, c_of))
+    return c_of[rank], g_of[rank], sums[rank], is_f[rank]
+
+
+def _ranked_lists(names, c_of, g_of, sums, is_float=None):
     """{contig: [(group, links), ...]} from arrays already ordered by (contig, rank)."""
     if len(c_of) == 0:
         return {}
     cuts = np.concatenate([[0], np.nonzero(np.diff(c_of))[0] + 1, [len(c_of)]])
     out = {}
-    g_list, s_list = g_of.tolist(), sums.tolist()
+    g_list, s_list = g_of.tolist(), _python_numbers(sums, is_float)
     for k in range(len(cuts) - 1):
         lo, hi = int(cuts[k]), int(cuts[k + 1])
         out[names[int(c_of[lo])]] = list(zip(g_list[lo:hi], s_list[lo:hi]))
@@ -1014,7 +1198,7 @@ def _best_group_statistics(fa_dict, link_dict, ctg_group, group_RE):
     zero = [(ctg, 0) for ctg in fa_dict]
     if arr is None:
         return zero, list(zero), list(zero)
-    gid, c_of, g_of, sums = arr
+    gid, c_of, g_of, sums, is_float = arr
     n_groups = len(group_RE)
     RE_g = np.array([group_RE[g] for g in range(int(gid.max()) + 1)], dtype=np.int64)
     RE_c = np.array([fa_dict[nm][2] for nm in names], dtype=np.int64)
@@ -1046,7 +1230,7 @@ def _best_group_statistics(fa_dict, link_dict, ctg_group, group_RE):
     with np.errstate(divide="ignore", invalid="ignore"):
         ratio = dens[starts] / others
     has = {int(c): k for k, c in enumerate(c_of[starts].tolist())}
-    top_links, top_dens = sums[starts].tolist(), dens[starts].tolist()
+    top_links, top_dens = _python_numbers(sums[starts], None if is_float is None else is_float[starts]), dens[starts].tolist()
     others_l, ratio_l = others.tolist(), ratio.tolist()
     name_idx = {nm: i for i, nm in enumerate(names)}
     best_links, best_density, best_ratio = [], [], []
@@ -1275,10 +1459,13 @@ def run(args, log_file=None):
     if args.correct_nrounds and args.ul:                   # 2774-2776
         args.ul = None
         logger.warning("Ultra-long data are not supported now when assembly correction is enabled")
-    unsupported = [("--ul", args.ul), ("--gfa", args.gfa)]
-    for flag, val in unsupported:
-        if val:
-            raise NotImplementedError("haphic_b200: {} is not supported (out of the hot-path scope)".format(flag))
+    if args.ul:
+        raise NotImplementedError("haphic_b200: --ul is not supported (out of the hot-path scope)")
+    gfa_list = args.gfa.split(",") if args.gfa else []
+    phasing = len(gfa_list) >= 2 and bool(args.phasing_weight)
+    if phasing and not 0 <= args.phasing_weight <= 1:
+        # the reference would turn inter-haplotype links into negative weights, which Markov clustering does not define
+        raise ValueError("--phasing_weight must lie in [0, 1], got {}".format(args.phasing_weight))
     if args.quick_view:
         args.bin_size = 0
         args.Nx = 100
@@ -1287,7 +1474,7 @@ def run(args, log_file=None):
 
     fa_dict = parse_fasta(args.fasta, RE=args.RE)
     pos_int_type, dist_int_type = determine_int_type(fa_dict)
-    read_depth_dict = dict()
+    read_depth_dict = parse_gfa(gfa_list, fa_dict) if gfa_list else dict()
     whitelist = set()
     args.whitelist = whitelist
     from . import hicio
@@ -1304,7 +1491,8 @@ def run(args, log_file=None):
         # the coverage pass, and its batches -- remapped to the corrected contigs -- feed the link counting (2835-2851)
         from . import correct
         alignments, _nbroken = correct.run_correction(_context(), fa_dict, args, open_alignments(False),
-                                                      lambda seq: count_RE_sites(seq, args.RE))
+                                                      lambda seq: count_RE_sites(seq, args.RE), read_depth_dict)
+    ctg_read_depth_dict = read_depth_dict.copy()            # contig level; stat_fragments moves read_depth_dict to bins
     _, bin_set, bin_size, frag_len_dict, Nx_frag_set, RE_site_dict, split_ctg_set = stat_fragments(
         fa_dict, args.RE, read_depth_dict, whitelist, nchrs=args.nchrs, flank=args.flank, Nx=args.Nx, bin_size=args.bin_size)
     if alignments is None:
@@ -1385,6 +1573,17 @@ def run(args, log_file=None):
         filtered_frags = remove_allelic_HiC_links(fa_dict, ctg_coord_dict, full_link_dict, args, flank_link_dict, filtered_frags,
                                                   ctg_pair_to_frag if split_ctg_set else None)
     del ctg_coord_dict
+    hap = None
+    if phasing:                                             # 2926-2928
+        # the matrix comes from the device table unless allelic removal edited the host dict: the table's matrix kernels
+        # then apply the same reduction to the flank links (hap per table fragment)
+        if flank_link_dict is not None:
+            reduce_inter_hap_HiC_links(flank_link_dict, read_depth_dict, args.phasing_weight, target="flank_link_dict")
+            if not args.remove_allelic_links:
+                hap = haplotype_array(read_depth_dict, names)
+        else:
+            hap = reduce_inter_hap_HiC_links(table, read_depth_dict, args.phasing_weight, target="flank_link_dict", names=names)
+        reduce_inter_hap_HiC_links(full_link_dict, ctg_read_depth_dict, args.phasing_weight, target="full_link_dict")
     if isinstance(full_link_dict, LinkArrays):
         logger.info("Writing {} to {}...".format("full_link_dict", "full_links.pkl"))
         full_link_dict.write_pickle("full_links.pkl")
@@ -1401,7 +1600,7 @@ def run(args, log_file=None):
         # dict_to_matrix on the device: first-seen indices from the table, unlinked fragments appended in
         # the reference's set-iteration order (355-359)
         link_matrix, frag_index_dict = device_matrix(table, names, filtered_frags, normalize_by_nlinks=args.normalize_by_nlinks,
-                                                     add_self_loops=True)
+                                                     add_self_loops=True, hap=hap, phasing_weight=args.phasing_weight)
     table.close()
     matrix_time = time.time()
     logger.info("Hi-C linking matrix was constructed in {}s".format(matrix_time - start_time))

@@ -152,9 +152,11 @@ def piece_names(ctg, points, length, unbroken):
     return ["{}:{}-{}".format(raw, bounds[k] + 1 + shift, bounds[k + 1] + shift) for k in range(len(bounds) - 1)]
 
 
-def break_and_update_ctgs(breaks, frag_source, final_pos, final_frag, fa_dict, unbroken, count_RE, new_ids=None):
+def break_and_update_ctgs(breaks, frag_source, final_pos, final_frag, fa_dict, unbroken, count_RE, new_ids=None,
+                          read_depth_dict=None):
     """The fa_dict / break-table part of break_and_update_ctgs (1115-1190).  ``breaks`` = [(ctg, [points])] in
-    ctg_break_point_dict order.  ``new_ids`` (list) receives the piece names in the order the device numbers them."""
+    ctg_break_point_dict order.  ``new_ids`` (list) receives the piece names in the order the device numbers them.  A
+    non-empty ``read_depth_dict`` (--gfa) gives every piece its parent's entry and loses the parent's (1147-1149, 1186-1187)."""
     logger.info("Breaking contigs and updating data...")
     for ctg, points in breaks:
         seq, length = fa_dict[ctg][0], fa_dict[ctg][1]
@@ -172,12 +174,16 @@ def break_and_update_ctgs(breaks, frag_source, final_pos, final_frag, fa_dict, u
             final_pos[source].insert(at, father_pos + s)
             piece = seq[s:e]
             fa_dict[name] = [piece, e - s, count_RE(piece)]   # no +1 pseudo-count here (1031)
+            if read_depth_dict:
+                read_depth_dict[name] = read_depth_dict[ctg]
             if new_ids is not None:
                 new_ids.append(name)
         del fa_dict[ctg]
+        if read_depth_dict:
+            del read_depth_dict[ctg]
 
 
-def correct_assembly(corr, fa_dict, args, count_RE):
+def correct_assembly(corr, fa_dict, args, count_RE, read_depth_dict=None):
     """correct_assembly (1200-1297) on a Correction whose coverage pass is done.  Mutates fa_dict; writes
     corrected_asm.fa and corrected_ctgs.txt; returns (nbroken_ctgs, final_break_pos_dict, final_break_frag_dict)."""
     logger.info("Performing assembly correction...")
@@ -206,17 +212,21 @@ def correct_assembly(corr, fa_dict, args, count_RE):
                 final_pos[ctg] = [0]
                 final_frag[ctg] = [ctg]
         new_ids = []
-        break_and_update_ctgs(breaks, frag_source, final_pos, final_frag, fa_dict, unbroken, count_RE, new_ids)
+        break_and_update_ctgs(breaks, frag_source, final_pos, final_frag, fa_dict, unbroken, count_RE, new_ids, read_depth_dict)
         if not last:
             assert len(frag_name) == int(info.n_frag)
             frag_name += new_ids
         unbroken -= {ctg for ctg, _ in breaks}
-    write_corrected_files(fa_dict, unbroken, nbroken, args.fasta)
+    gfa_list = args.gfa.split(",") if args.gfa else []
+    write_corrected_files(fa_dict, unbroken, nbroken, args.fasta,
+                          read_depth_dict, gfa_list if args.quick_view and read_depth_dict and len(gfa_list) >= 2 else None)
     return nbroken, final_pos, final_frag
 
 
-def write_corrected_files(fa_dict, unbroken, nbroken, fasta):
-    """corrected_asm.fa / corrected_ctgs.txt (1252-1290); an existing corrected_asm.fa is renamed first."""
+def write_corrected_files(fa_dict, unbroken, nbroken, fasta, read_depth_dict=None, gfa_list=None):
+    """corrected_asm.fa / corrected_ctgs.txt (1252-1290); an existing corrected_asm.fa is renamed first.  With ``gfa_list``
+    (quick view with >= 2 GFA files) also corrected_<GFA basename> per haplotype for `haphic reassign`: the S lines of the
+    corrected contigs of that haplotype in read_depth_dict order, or a symlink to the GFA when nothing was broken."""
     asm_file, list_file = "corrected_asm.fa", "corrected_ctgs.txt"
     logger.info("Generating corrected assembly file...")
     if os.path.exists(asm_file):
@@ -233,11 +243,18 @@ def write_corrected_files(fa_dict, unbroken, nbroken, fasta):
             for ctg in fa_dict:
                 if ctg not in unbroken:
                     f.write(ctg + "\n")
+        for hap, gfa in enumerate(gfa_list or ()):
+            with open("corrected_" + os.path.basename(gfa), "w") as f:
+                for ctg, (h, depth) in read_depth_dict.items():
+                    if h == hap:
+                        f.write("S\t{}\t*\tLN:i:{}\trd:i:{}\n".format(ctg, fa_dict[ctg][1], depth))
     else:
         logger.info("No corrected contigs were found. Simply create a symbolic link of the input assembly")
         os.symlink(fasta, asm_file)
         with open(list_file, "w"):
             pass
+        for gfa in gfa_list or ():
+            os.symlink(gfa, "corrected_" + os.path.basename(gfa))
 
 
 def remap_layout(src_names, fa_dict, final_pos, final_frag):
@@ -257,7 +274,7 @@ def remap_layout(src_names, fa_dict, final_pos, final_frag):
     return np.asarray(base, np.int32), np.asarray(starts, np.int64), np.asarray(ids, np.int32)
 
 
-def run_correction(ctx, fa_dict, args, batches, count_RE):
+def run_correction(ctx, fa_dict, args, batches, count_RE, read_depth_dict=None):
     """The whole correction step of run() (2798-2808, 2835-2851): one read of the alignments feeds the coverage pass;
     returns (record batches for link counting, nbroken_ctgs).  The batches are remapped to the corrected contigs when
     anything was broken, else returned as read."""
@@ -268,7 +285,7 @@ def run_correction(ctx, fa_dict, args, batches, count_RE):
             kept = parse_bam_for_correction(corr, batches)
         else:
             kept = parse_pairs_for_correction(corr, batches)
-        nbroken, final_pos, final_frag = correct_assembly(corr, fa_dict, args, count_RE)
+        nbroken, final_pos, final_frag = correct_assembly(corr, fa_dict, args, count_RE, read_depth_dict)
         if nbroken:
             corr.set_layout(*remap_layout(src_names, fa_dict, final_pos, final_frag))
             kept = [corr.remap(rec, in_place=True) for rec in kept]

@@ -1039,7 +1039,8 @@ extern "C" int hh_clm_from_records(const char* path, const char* names_blob, int
 // full_links.pkl / HT_links.pkl (output_pickle, 710-715) without building the Python dicts: a pickle stream
 // (protocol 3 opcodes) that loads as `defaultdict(int, {(name_i, name_j): value, ...})` in entry order.
 // Strings are memoised like pickle does, so the loaded keys share one str object per contig.
-//   mode 0: one entry per pair, value = values_i64[e] (or values_f64[e] when given);
+//   mode 0: one entry per pair, value = values_i64[e] (or values_f64[e] when given; with is_float, entry e is a float
+//           when is_float[e] and the int (int64_t)values_f64[e] otherwise -- the mixed dict of a fractional phasing weight);
 //   mode 1: HT_link_dict -- ht[e][4] = {HH, HT, TH, TT}; non-zero counters become the keys
 //           (name_i + '_H'|'_T', name_j + '_H'|'_T') (update_HT_link_dict, 404-416).
 // ---------------------------------------------------------------------------------------------
@@ -1106,8 +1107,9 @@ struct pickle_out {
 };
 }   // namespace
 
-extern "C" int hh_pickle_links(const char* path, const char* names_blob, int32_t n_names, const int32_t* key_i, const int32_t* key_j,
-                               int64_t n_entries, const int64_t* values_i64, const double* values_f64, const uint32_t* ht) {
+static int pickle_links(const char* path, const char* names_blob, int32_t n_names, const int32_t* key_i, const int32_t* key_j,
+                        int64_t n_entries, const int64_t* values_i64, const double* values_f64, const uint8_t* is_float,
+                        const uint32_t* ht) {
     if (!path || !names_blob || n_names <= 0 || n_entries < 0 || (n_entries > 0 && (!key_i || !key_j)) ||
         (n_entries > 0 && !values_i64 && !values_f64 && !ht)) {
         hh_set_error("hh_pickle_links: bad argument");
@@ -1182,8 +1184,8 @@ extern "C" int hh_pickle_links(const char* path, const char* names_blob, int32_t
             key_string(a, -1);
             key_string(b, -1);
             o.byte(0x86);
-            if (values_f64) o.real(values_f64[e]);
-            else o.integer(values_i64[e]);
+            if (values_f64 && (!is_float || is_float[e])) o.real(values_f64[e]);
+            else o.integer(values_f64 ? (int64_t)values_f64[e] : values_i64[e]);
             ++in_batch;
             close_batch(false);
         } else {
@@ -1208,6 +1210,20 @@ extern "C" int hh_pickle_links(const char* path, const char* names_blob, int32_t
         return HH_ERR_ARG;
     }
     return HH_OK;
+}
+
+extern "C" int hh_pickle_links(const char* path, const char* names_blob, int32_t n_names, const int32_t* key_i, const int32_t* key_j,
+                               int64_t n_entries, const int64_t* values_i64, const double* values_f64, const uint32_t* ht) {
+    return pickle_links(path, names_blob, n_names, key_i, key_j, n_entries, values_i64, values_f64, nullptr, ht);
+}
+
+extern "C" int hh_pickle_links_mixed(const char* path, const char* names_blob, int32_t n_names, const int32_t* key_i,
+                                     const int32_t* key_j, int64_t n_entries, const double* values, const uint8_t* is_float) {
+    if (n_entries > 0 && (!values || !is_float)) {
+        hh_set_error("hh_pickle_links_mixed: bad argument");
+        return HH_ERR_ARG;
+    }
+    return pickle_links(path, names_blob, n_names, key_i, key_j, n_entries, nullptr, values, is_float, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

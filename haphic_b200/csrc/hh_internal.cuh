@@ -13,6 +13,28 @@ struct hh_matrix {
     int32_t n_index;
 };
 
+// How the matrix sees one entry of the compact link table (9 x uint32: i, j, full, flank, ...): the flank count, or
+// links / (tot_i * tot_j) ** 0.5 in fp64 with normalize (normalize_by_nlinks, 718-724), then -- when hap != NULL and the
+// two ends lie on different haplotypes -- x - x * w with two roundings (reduce_inter_hap_HiC_links, 695-707).  Returns
+// false when the entry is not in the (reduced) flank_link_dict: no flank link, or reduced to exactly 0.  hh_k_touch,
+// hh_k_mat_count and hh_k_mat_scatter all decide through this one function, so pattern, values and first-seen indices
+// cannot disagree.
+__device__ __forceinline__ bool hh_flank_value(const uint32_t* __restrict__ p, const unsigned long long* __restrict__ ctg_tot,
+                                               int normalize, const int32_t* __restrict__ hap, double w, double* x_out) {
+    if (p[3] == 0) return false;
+    double x;
+    if (normalize) {
+        const unsigned long long prod = ctg_tot[p[0]] * ctg_tot[p[1]];
+        x = (double)p[3] / pow((double)prod, 0.5);
+    } else {
+        x = (double)p[3];
+    }
+    if (hap != nullptr && hap[p[0]] != hap[p[1]]) x = __dsub_rn(x, __dmul_rn(x, w));
+    if (x == 0.0) return false;
+    *x_out = x;
+    return true;
+}
+
 // hh_links accessors (hh_links.cu)
 int32_t hh_links_n_ctg(hh_links* lk);
 hh_ctx* hh_links_ctx(hh_links* lk);
@@ -21,3 +43,4 @@ const unsigned long long* hh_links_ctg_totals(hh_links* lk);
 int32_t* hh_links_index_dev(hh_links* lk, int32_t* n_linked);
 uint8_t* hh_links_keep_dev(hh_links* lk);
 bool hh_links_finished(hh_links* lk);
+const int32_t* hh_links_hap_dev(hh_links* lk);   // haplotypes of the last phased hh_links_linked_index_phased; NULL = none

@@ -15,6 +15,7 @@
 // hh_links_finish orders the distinct keys by first appearance with a scatter + stream
 // compaction (no sort): order[first_full] = slot, then compact.
 #include "hh_common.cuh"
+#include "hh_internal.cuh"
 #include <stdlib.h>
 #include <vector>
 
@@ -89,6 +90,8 @@ struct hh_links {
     int32_t* d_index;                // [n_ctg] matrix index of linked fragments (hh_links_linked_index)
     int32_t n_linked;
     uint8_t* d_keep;
+    int32_t* d_hap;                  // [n_ctg] haplotype of every fragment (allocated on the first phased call)
+    bool phased;                     // the last hh_links_linked_index_phased got a haplotype array
 };
 
 __device__ __forceinline__ uint64_t hh_mix64(uint64_t k) {
@@ -731,16 +734,20 @@ hh_k_compact_gather(const uint32_t* __restrict__ order, int64_t n, const int64_t
 }
 
 // ---------------------------------------------------------------------------------------------
-// dict_to_matrix index assignment (327-349): first touch of each fragment in flank-dict order
+// dict_to_matrix index assignment (327-349): first touch of each fragment in flank-dict order.  An entry that the
+// phasing reduction deleted is not in the dict and touches nothing.
 // ---------------------------------------------------------------------------------------------
 __global__ void hh_k_touch(const uint32_t* __restrict__ compact, int64_t nnz, const uint8_t* __restrict__ keep,
-                           unsigned long long* __restrict__ touch) {
+                           const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
+                           double w, unsigned long long* __restrict__ touch) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
         const uint32_t* p = compact + e * 9;
-        if (p[3] == 0) continue;                       // not in flank_link_dict
+        if (p[3] == 0) continue;                       // no flank link
         const uint32_t i = p[0], j = p[1];
         if (!keep[i] || !keep[j]) continue;            // 329-330
+        double x;
+        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;   // not in flank_link_dict
         const unsigned long long t = (unsigned long long)p[5] * 2ull;
         atomicMin(touch + i, t);
         atomicMin(touch + j, t + 1ull);
@@ -1559,11 +1566,22 @@ extern "C" int hh_links_merge(hh_links* lk, const uint32_t* entries_dev, int64_t
 }
 
 extern "C" int hh_links_linked_index(hh_links* lk, const uint8_t* keep, int32_t* index, int32_t* n_linked) {
+    return hh_links_linked_index_phased(lk, keep, 0, nullptr, 0.0, index, n_linked);
+}
+
+extern "C" int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, int normalize_by_nlinks, const int32_t* hap,
+                                            double w, int32_t* index, int32_t* n_linked) {
     HH_REQUIRE(lk && keep, HH_ERR_ARG, "hh_links_linked_index: NULL argument");
     hh_scope _scope(lk->ctx);
     HH_REQUIRE(lk->finished, HH_ERR_STATE, "hh_links_linked_index: call hh_links_finish first");
+    HH_REQUIRE(!hap || (w >= 0.0 && w <= 1.0), HH_ERR_ARG, "hh_links_linked_index_phased: phasing weight %g outside [0, 1]", w);
     hh_ctx* ctx = lk->ctx;
     HH_CUDA(cudaSetDevice(ctx->device));
+    lk->phased = hap != nullptr;
+    if (hap) {
+        if (!lk->d_hap) HH_CHECK(hh_dmalloc(&lk->d_hap, (size_t)lk->n_ctg));
+        HH_CUDA(cudaMemcpyAsync(lk->d_hap, hap, (size_t)lk->n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    }
     unsigned long long* d_touch = nullptr;
     HH_CHECK(hh_dmalloc(&d_touch, (size_t)lk->n_ctg));
     int rc = [&]() -> int {
@@ -1574,7 +1592,8 @@ extern "C" int hh_links_linked_index(hh_links* lk, const uint8_t* keep, int32_t*
         if (lk->nnz) {
             int64_t blocks = (lk->nnz + 255) / 256;
             int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
-            HH_LAUNCH(ctx, hh_k_touch, grid, 256, 0, lk->d_compact, lk->nnz, lk->d_keep, d_touch);
+            HH_LAUNCH(ctx, hh_k_touch, grid, 256, 0, lk->d_compact, lk->nnz, lk->d_keep, lk->d_ctg, normalize_by_nlinks,
+                      hh_links_hap_dev(lk), w, d_touch);
         }
         HH_LAUNCH(ctx, hh_k_rank_touch, (lk->n_ctg + 255) / 256, 256, 0, d_touch, lk->n_ctg, lk->d_index, d_nl);
         HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 8, d_nl, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1616,6 +1635,7 @@ extern "C" int hh_links_destroy(hh_links* lk) {
     hh_dfree(lk->d_compact);
     hh_dfree(lk->d_index);
     hh_dfree(lk->d_keep);
+    hh_dfree(lk->d_hap);
     links_free_partsets(lk);
     delete lk->psets;
     delete lk;
@@ -1630,3 +1650,4 @@ const unsigned long long* hh_links_ctg_totals(hh_links* lk) { return lk->d_ctg; 
 int32_t* hh_links_index_dev(hh_links* lk, int32_t* n_linked) { *n_linked = lk->n_linked; return lk->d_index; }
 uint8_t* hh_links_keep_dev(hh_links* lk) { return lk->d_keep; }
 bool hh_links_finished(hh_links* lk) { return lk->finished; }
+const int32_t* hh_links_hap_dev(hh_links* lk) { return lk->phased ? lk->d_hap : nullptr; }

@@ -1,5 +1,6 @@
 // dict_to_matrix (scripts/HapHiC_cluster.py:310-373) on the GPU: from the compact link table to a
-// symmetric fp32 CSC with self loops, in the reference's first-seen index order.
+// symmetric fp32 CSC with self loops, in the reference's first-seen index order.  With a haplotype array the
+// inter-haplotype entries are reduced first (reduce_inter_hap_HiC_links, 695-707; hh_flank_value).
 #include "hh_common.cuh"
 #include "hh_internal.cuh"
 
@@ -25,13 +26,16 @@ __global__ void hh_k_check_index(const int32_t* __restrict__ index, const uint8_
 }
 
 __global__ void hh_k_mat_count(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
-                               int* __restrict__ colcnt) {
+                               const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
+                               double w, int* __restrict__ colcnt) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
         const uint32_t* p = compact + e * 9;
         if (p[3] == 0) continue;
         const int ii = index[p[0]], jj = index[p[1]];
         if (ii < 0 || jj < 0) continue;                 // 329-330
+        double x;
+        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
         atomicAdd(colcnt + ii, 1);
         atomicAdd(colcnt + jj, 1);
     }
@@ -43,23 +47,18 @@ __global__ void hh_k_fill_i32(int* __restrict__ p, int v, int n) {
 }
 
 __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
-                                 const unsigned long long* __restrict__ ctg_tot, int normalize,
-                                 const int64_t* __restrict__ colptr, int* __restrict__ cursor, int32_t* __restrict__ row,
-                                 float* __restrict__ val) {
+                                 const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
+                                 double w, const int64_t* __restrict__ colptr, int* __restrict__ cursor,
+                                 int32_t* __restrict__ row, float* __restrict__ val) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
         const uint32_t* p = compact + e * 9;
         if (p[3] == 0) continue;
         const int ii = index[p[0]], jj = index[p[1]];
         if (ii < 0 || jj < 0) continue;
-        float v;
-        if (normalize) {
-            // links / (tot_i * tot_j) ** 0.5 in fp64 (718-724), cast to fp32 by coo_matrix(dtype=float32) (368)
-            const unsigned long long prod = ctg_tot[p[0]] * ctg_tot[p[1]];
-            v = (float)((double)p[3] / pow((double)prod, 0.5));
-        } else {
-            v = (float)p[3];
-        }
+        double x;
+        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
+        const float v = (float)x;                      // coo_matrix(dtype=float32) (368)
         int64_t q = colptr[jj] + atomicAdd(cursor + jj, 1);    // (row ii, col jj)
         row[q] = ii;
         val[q] = v;
@@ -97,6 +96,12 @@ static int matrix_alloc(hh_ctx* ctx, int32_t n, int64_t nnz, hh_matrix** out) {
 
 extern "C" int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
                                     int normalize_by_nlinks, int add_self_loops, hh_matrix** out) {
+    return hh_matrix_from_links_phased(lk, keep, tail, n_tail, normalize_by_nlinks, add_self_loops, nullptr, 0.0, out);
+}
+
+extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
+                                           int normalize_by_nlinks, int add_self_loops, const int32_t* hap, double w,
+                                           hh_matrix** out) {
     HH_REQUIRE(lk && keep && out, HH_ERR_ARG, "hh_matrix_from_links: NULL argument");
     hh_scope _scope(hh_links_ctx(lk));
     HH_REQUIRE(n_tail >= 0 && (tail || n_tail == 0), HH_ERR_ARG, "hh_matrix_from_links: bad tail");
@@ -107,7 +112,8 @@ extern "C" int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int
     const int n_ctg = hh_links_n_ctg(lk);
     // (re)compute the first-seen indices for this keep mask
     int32_t n_linked = 0;
-    HH_CHECK(hh_links_linked_index(lk, keep, nullptr, &n_linked));
+    HH_CHECK(hh_links_linked_index_phased(lk, keep, normalize_by_nlinks, hap, w, nullptr, &n_linked));
+    const int32_t* d_hap = hh_links_hap_dev(lk);
     int32_t* d_index = hh_links_index_dev(lk, &n_linked);
     const uint8_t* d_keep = hh_links_keep_dev(lk);
     const int n = n_linked + n_tail;
@@ -132,7 +138,8 @@ extern "C" int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int
         int64_t nnz_c = 0;
         const uint32_t* compact = hh_links_compact(lk, &nnz_c);
         const int gridc = (int)((nnz_c + 255) / 256 < (int64_t)ctx->sm_count * 8 ? (nnz_c + 255) / 256 : (int64_t)ctx->sm_count * 8);
-        if (nnz_c) HH_LAUNCH(ctx, hh_k_mat_count, gridc, 256, 0, compact, nnz_c, d_index, d_cnt);
+        if (nnz_c) HH_LAUNCH(ctx, hh_k_mat_count, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk),
+                              normalize_by_nlinks, d_hap, w, d_cnt);
         int64_t* d_ptr = nullptr;
         HH_CHECK(hh_dmalloc(&d_ptr, (size_t)n + 1));
         int rc2 = [&]() -> int {
@@ -149,7 +156,7 @@ extern "C" int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int
             HH_CUDA(cudaMemcpyAsync(m->d_colptr, d_ptr, ((size_t)n + 1) * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
             if (nnz_c)
                 HH_LAUNCH(ctx, hh_k_mat_scatter, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks,
-                          m->d_colptr, d_cursor, m->d_row, m->d_val);
+                          d_hap, w, m->d_colptr, d_cursor, m->d_row, m->d_val);
             if (add_self_loops) HH_LAUNCH(ctx, hh_k_mat_diag, (n + 255) / 256, 256, 0, n, m->d_colptr, d_cursor, m->d_row, m->d_val);
             HH_CHECK(hh_dmalloc(&m->d_index, (size_t)n_ctg));
             m->n_index = n_ctg;

@@ -135,25 +135,41 @@ class LinkTable:
         check(load().hh_links_fetch_ctg(self._h, ptr(tot)))
         return tot
 
-    def linked_index(self, keep):
+    def _hap(self, hap):
+        if hap is None:
+            return None
+        hap = np.ascontiguousarray(hap, dtype=np.int32)
+        if hap.shape != (self.n_ctg,):
+            raise ValueError("hap must have one entry per fragment of the table")
+        return hap
+
+    def linked_index(self, keep, hap=None, phasing_weight: float = 0.0, normalize_by_nlinks: bool = False):
         """(index, n_linked): first-seen matrix index of every fragment present in
-        flank_link_dict restricted to ``keep`` (HapHiC_cluster.py:327-349); -1 elsewhere."""
+        flank_link_dict restricted to ``keep`` (HapHiC_cluster.py:327-349); -1 elsewhere.  With ``hap`` (haplotype index
+        per fragment) the dict is the one reduce_inter_hap_HiC_links (695-707) leaves for ``phasing_weight``."""
         if self.info is None:
             self.finish()
         keep = np.ascontiguousarray(keep, dtype=np.uint8)
+        hap = self._hap(hap)
         index = np.empty(self.n_ctg, np.int32)
         n_linked = C.c_int32()
-        check(load().hh_links_linked_index(self._h, ptr(keep), ptr(index), C.byref(n_linked)))
+        check(load().hh_links_linked_index_phased(self._h, ptr(keep), int(bool(normalize_by_nlinks)),
+                                                  ptr(hap) if hap is not None else None, float(phasing_weight), ptr(index),
+                                                  C.byref(n_linked)))
         return index, int(n_linked.value)
 
-    def to_matrix(self, keep, tail=None, normalize_by_nlinks: bool = False, add_self_loops: bool = True) -> "LinkMatrix":
+    def to_matrix(self, keep, tail=None, normalize_by_nlinks: bool = False, add_self_loops: bool = True, hap=None,
+                  phasing_weight: float = 0.0) -> "LinkMatrix":
+        """dict_to_matrix on the device; ``hap`` / ``phasing_weight`` as in linked_index."""
         if self.info is None:
             self.finish()
         keep = np.ascontiguousarray(keep, dtype=np.uint8)
         tail = np.ascontiguousarray(tail if tail is not None else [], dtype=np.int32)
+        hap = self._hap(hap)
         h = C.c_void_p()
-        check(load().hh_matrix_from_links(self._h, ptr(keep), ptr(tail) if len(tail) else None, len(tail),
-                                          int(bool(normalize_by_nlinks)), int(bool(add_self_loops)), C.byref(h)))
+        check(load().hh_matrix_from_links_phased(self._h, ptr(keep), ptr(tail) if len(tail) else None, len(tail),
+                                                 int(bool(normalize_by_nlinks)), int(bool(add_self_loops)),
+                                                 ptr(hap) if hap is not None else None, float(phasing_weight), C.byref(h)))
         return LinkMatrix(self.ctx, h)
 
     # -- multi-GPU -------------------------------------------------------------------------

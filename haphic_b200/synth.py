@@ -264,3 +264,71 @@ def chimera_case(nchr: int, n_contigs: int, mean_len: int, n_pairs: int, n_joins
     for k in range(len(joins2)):
         a2.names[-(len(joins2) - k)] = "chimera{}".format(n_joins // 2 + k + 1)
     return a2, p2, [(moved[c], pos) for c, pos in j1] + j2
+
+
+def write_gfa(asm: Assembly, paths, seed: int = 12345, depth: int = 30, collapsed: int = 4, extra=(), hap=None,
+              ploidy=None) -> np.ndarray:
+    """hifiasm-style GFA files of a haplotype-resolved assembly, one per haplotype: contig c belongs to haplotype
+    ``hap[c]`` (default ``chrom[c] % ploidy``, the layout of make_pairs(homolog=(ploidy, ...)); ploidy defaults to
+    ``len(paths)``) and goes to file ``hap[c] % len(paths)`` -- one file holds every contig -- as an ``S name * LN:i: rd:i:``
+    line followed by one ``A`` line; every file ends with ``L`` lines between its consecutive contigs.  Read depths are
+    ``depth`` +- 20 %, except for ``collapsed`` contigs at 2-3x (collapsed repeats, the outliers of the read-depth filter).
+    ``extra`` names contigs written to the first file only (GFA segments missing from the FASTA).  Returns the depths."""
+    rng = np.random.default_rng(seed)
+    nfile = len(paths)
+    ploidy = ploidy or nfile
+    if hap is None:
+        hap = asm.chrom.astype(np.int64) % ploidy
+    rd = rng.integers(int(depth * 0.8), int(depth * 1.2) + 1, size=asm.n)
+    if collapsed:
+        pick = rng.choice(asm.n, size=min(collapsed, asm.n), replace=False)
+        rd[pick] *= rng.integers(2, 4, size=len(pick))
+    files = [open(p, "w") for p in paths]
+    try:
+        for f in files:
+            f.write("H\tVN:Z:1.0\n")
+        last = [None] * nfile
+        links = [[] for _ in range(nfile)]
+        for c, (name, ln) in enumerate(zip(asm.names, asm.lengths.tolist())):
+            h = int(hap[c]) % nfile
+            files[h].write("S\t{}\t*\tLN:i:{}\trd:i:{}\n".format(name, ln, int(rd[c])))
+            files[h].write("A\t{}\t0\t+\tread{}\t0\t{}\tid:i:{}\tHG:A:*\n".format(name, c, min(ln, 20000), c))
+            if last[h] is not None:
+                links[h].append("L\t{}\t+\t{}\t+\t0M\tL1:i:{}\n".format(last[h], name, ln))
+            last[h] = name
+        for k, name in enumerate(extra):
+            files[0].write("S\t{}\t*\tLN:i:{}\trd:i:{}\n".format(name, 10000 + k, depth))
+        for f, ls in zip(files, links):
+            f.writelines(ls)
+    finally:
+        for f in files:
+            f.close()
+    return rd
+
+
+def gfa_case(nchr, n_contigs, mean_len, n_pairs, seed, ploidy, n_gfa, chimeras, out_dir, bam=False):
+    """A seeded haplotype-resolved input set for `haphic cluster --gfa` in ``out_dir``: asm.fa, aln.pairs (or aln.bam) and
+    h1.gfa .. h{n_gfa}.gfa.  ``nchr`` chromosomes form nchr / ploidy homologous groups (make_pairs(homolog=(ploidy, 0.2)));
+    ``chimeras`` > 0 joins that many pairs of contigs of one haplotype (for --correct_nrounds).  Returns the GFA paths."""
+    import os
+    asm = make_assembly(nchr, n_contigs, mean_len, seed=seed)
+    pairs = make_pairs(asm, n_pairs, seed=seed + 1, homolog=(ploidy, 0.2)).numpy()
+    hap = None
+    if chimeras:
+        rng = np.random.default_rng(seed + 2)
+        per = asm.n // nchr
+        joins = [(int(c), int(c) + per * ploidy) for c in rng.permutation(per)[:chimeras]]
+        joined = {x for j in joins for x in j}
+        # make_chimeras keeps the other contigs in order and appends the chimeras
+        hap = np.array([int(asm.chrom[c]) % ploidy for c in range(asm.n) if c not in joined]
+                       + [int(asm.chrom[j[0]]) % ploidy for j in joins], np.int32)
+        asm, pairs, _ = make_chimeras(asm, pairs, joins, seed=seed + 3, gap=1000)
+    write_fasta(asm, os.path.join(out_dir, "asm.fa"), seed=seed + 3)
+    if bam:
+        from . import hicio
+        hicio.write_bam(os.path.join(out_dir, "aln.bam"), asm.names, asm.lengths.tolist(), pairs)
+    else:
+        write_pairs(asm, pairs, os.path.join(out_dir, "aln.pairs"))
+    gfa = [os.path.join(out_dir, "h{}.gfa".format(k + 1)) for k in range(n_gfa)]
+    write_gfa(asm, gfa, seed=seed + 4, hap=hap, ploidy=ploidy)
+    return gfa

@@ -155,6 +155,16 @@ int hh_links_destroy(hh_links* lk);
 int hh_links_linked_index(hh_links* lk, const uint8_t* keep, int32_t* index, int32_t* n_linked);
 int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
                          int normalize_by_nlinks, int add_self_loops, hh_matrix** out);
+/* The same two steps on the phasing-reduced flank_link_dict (reduce_inter_hap_HiC_links, 695-707, with --gfa of >= 2
+ * haplotype files): hap[n_ctg] (host) is the haplotype index of every fragment of the table's id space, w in [0, 1] the
+ * phasing weight.  An entry whose ends differ in hap becomes x - x * w (fp64, two roundings; x = the flank count, or the
+ * normalised value when normalize_by_nlinks) and is absent when that is exactly 0: it then sets no first-seen index and no
+ * matrix entry.  hap = NULL is the unphased call above (which is this one with hap = NULL); hh_matrix_from_links_phased
+ * recomputes the indices with its own arguments, so give both calls the same keep / normalize_by_nlinks / hap / w. */
+int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, int normalize_by_nlinks, const int32_t* hap, double w,
+                                 int32_t* index, int32_t* n_linked);
+int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
+                                int normalize_by_nlinks, int add_self_loops, const int32_t* hap, double w, hh_matrix** out);
 /* rank-sum statistic of filter_fragments, HapHiC_cluster.py:864-892, on a matrix WITHOUT self loops: for every
  * fragment, sort its row by links descending (ties by matrix index, a stable list.sort(reverse=True)), take
  * the first topN fragments and sum min(rank_a(b), rank_b(a)) over their pairs.  rank_sum[n] (host) is
@@ -350,6 +360,10 @@ int hh_clm_from_records(const char* path, const char* names_blob, int32_t n_name
  * keys are (name_i + '_H'|'_T', name_j + '_H'|'_T') for the non-zero counters (update_HT_link_dict, 404-416). */
 int hh_pickle_links(const char* path, const char* names_blob, int32_t n_names, const int32_t* key_i, const int32_t* key_j,
                     int64_t n_entries, const int64_t* values_i64, const double* values_f64, const uint32_t* ht);
+/* full_links.pkl after a fractional phasing weight: reduced entries are Python floats, the others stay ints.  Entry e is
+ * written as the float values[e] when is_float[e], else as the int (int64_t)values[e]. */
+int hh_pickle_links_mixed(const char* path, const char* names_blob, int32_t n_names, const int32_t* key_i, const int32_t* key_j,
+                          int64_t n_entries, const double* values, const uint8_t* is_float);
 
 #ifdef __cplusplus
 }
