@@ -97,6 +97,7 @@ _SIGNATURES = {
                               C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     "hh_mcl_fetch_m0": (C.c_int, [_P, _P, _P, _P]),
     "hh_mcl_fetch_m1": (C.c_int, [_P, _P]),
+    "hh_mcl_fetch_m1_cols": (C.c_int, [_P, C.c_int32, C.c_int32, _P]),
     "hh_mcl_run": (C.c_int, [_P, C.c_double, C.c_int, C.c_double, C.POINTER(MclResult), _P, _P, _P, _P]),
     "hh_mcl_fetch_result": (C.c_int, [_P, _P, _P, _P]),
     "hh_mcl_begin": (C.c_int, [_P, C.c_double, C.c_double]),

@@ -2549,14 +2549,21 @@ extern "C" int hh_mcl_fetch_m0(hh_mcl* mc, int64_t* indptr, int32_t* indices, fl
     return slot_fetch_csc(mc->ctx, mc->m0, 0, mc->n, indptr, indices, data);
 }
 
-extern "C" int hh_mcl_fetch_m1(hh_mcl* mc, float* dense) {
-    HH_REQUIRE(mc && dense, HH_ERR_ARG, "hh_mcl_fetch_m1: NULL argument");
+extern "C" int hh_mcl_fetch_m1_cols(hh_mcl* mc, int32_t col_lo, int32_t col_hi, float* dense) {
+    HH_REQUIRE(mc && dense, HH_ERR_ARG, "hh_mcl_fetch_m1_cols: NULL argument");
+    HH_REQUIRE(mc->own_lo <= col_lo && col_lo < col_hi && col_hi <= mc->own_hi, HH_ERR_ARG,
+               "hh_mcl_fetch_m1_cols: columns [%d, %d) are not inside the owned block [%d, %d)", col_lo, col_hi, mc->own_lo, mc->own_hi);
     HH_CUDA(cudaSetDevice(mc->ctx->device));
-    const int ncols = mc->own_hi - mc->own_lo;
-    HH_CUDA(cudaMemcpy2DAsync(dense, (size_t)mc->n * sizeof(float), mc->d_m1, (size_t)mc->ld * sizeof(float),
-                              (size_t)mc->n * sizeof(float), (size_t)ncols, cudaMemcpyDeviceToHost, mc->ctx->stream));
+    const float* src = mc->d_m1 + (size_t)(col_lo - mc->own_lo) * (size_t)mc->ld;
+    HH_CUDA(cudaMemcpy2DAsync(dense, (size_t)mc->n * sizeof(float), src, (size_t)mc->ld * sizeof(float),
+                              (size_t)mc->n * sizeof(float), (size_t)(col_hi - col_lo), cudaMemcpyDeviceToHost, mc->ctx->stream));
     HH_CUDA(cudaStreamSynchronize(mc->ctx->stream));
     return HH_OK;
+}
+
+extern "C" int hh_mcl_fetch_m1(hh_mcl* mc, float* dense) {
+    HH_REQUIRE(mc && dense, HH_ERR_ARG, "hh_mcl_fetch_m1: NULL argument");
+    return hh_mcl_fetch_m1_cols(mc, mc->own_lo, mc->own_hi, dense);
 }
 
 // components of the committed iterate's pattern -> perm / inv / component windows / column lists, then the

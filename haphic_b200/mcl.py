@@ -61,11 +61,13 @@ class Mcl:
     def m0(self):
         return self._fetch_csc(load().hh_mcl_fetch_m0)
 
-    def m1(self) -> np.ndarray:
-        """Owned block of the pre-expanded matrix, dense [n, col_hi-col_lo] (column-major on device)."""
-        ncols = self.col_hi - self.col_lo
-        buf = np.empty((ncols, self.n), np.float32)
-        check(load().hh_mcl_fetch_m1(self._h, ptr(buf)))
+    def m1(self, col_lo: int | None = None, col_hi: int | None = None) -> np.ndarray:
+        """Columns [col_lo, col_hi) of the pre-expanded matrix (default: the owned block), dense [n, col_hi-col_lo]
+        (column-major on device)."""
+        lo = self._own[0] if col_lo is None else int(col_lo)
+        hi = self._own[1] if col_hi is None else int(col_hi)
+        buf = np.empty((max(hi - lo, 0), self.n), np.float32)
+        check(load().hh_mcl_fetch_m1_cols(self._h, lo, hi, ptr(buf)))
         return buf.T
 
     # -- one mcl() call on a single GPU ----------------------------------------------------------

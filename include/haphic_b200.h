@@ -220,6 +220,8 @@ int hh_mcl_info(hh_mcl* mc, int32_t* n, int64_t* nnz_m0, int64_t* preexp_product
 /* M0 as canonical CSC / owned block of M1 as dense column-major fp32 [n * (col_hi-col_lo)] */
 int hh_mcl_fetch_m0(hh_mcl* mc, int64_t* indptr, int32_t* indices, float* data);
 int hh_mcl_fetch_m1(hh_mcl* mc, float* dense);
+/* columns [col_lo, col_hi) of M1 (absolute indices inside the owned block), dense column-major fp32 [n * (col_hi-col_lo)] */
+int hh_mcl_fetch_m1_cols(hh_mcl* mc, int32_t col_lo, int32_t col_hi, float* dense);
 
 typedef struct {
     int32_t rounds;          /* iterations executed ("after N rounds", 2047-2060)          */
