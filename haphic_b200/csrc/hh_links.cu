@@ -947,6 +947,29 @@ static int links_new_partset(hh_links* lk, int64_t n_rec) {
     return HH_OK;
 }
 
+// the spill list holds an eighth of the records the partition sets are sized for, plus 4 Mi.  It is sized with the first
+// set and grown when a later call opens another one, so that a stream sent in several calls spills into as much room as the
+// same stream sent in one.  The copy of the old list is ordered on the library stream behind every scatter that wrote it
+// and ahead of the next one; the spill cursor is unchanged.
+static int links_size_spill(hh_links* lk) {
+    int64_t sized = 0;
+    for (size_t k = 0; k < lk->psets->size(); ++k) sized += (*lk->psets)[k].sized_for;
+    const uint64_t need = (uint64_t)(sized / 8) + (4u << 20);
+    if (lk->d_spill && need <= lk->spill_cap) return HH_OK;
+    int4* grown = nullptr;
+    HH_CHECK(hh_ws_alloc(lk->ctx, &grown, (size_t)need));
+    if (lk->d_spill) {
+        const cudaError_t e = cudaMemcpyAsync(grown, lk->d_spill, (size_t)lk->spill_cap * sizeof(int4), cudaMemcpyDeviceToDevice,
+                                              lk->ctx->stream);
+        if (e != cudaSuccess) hh_ws_free(lk->ctx, grown);
+        HH_CUDA(e);
+        hh_ws_free(lk->ctx, lk->d_spill);
+    }
+    lk->d_spill = grown;
+    lk->spill_cap = need;
+    return HH_OK;
+}
+
 // first records of the stream: direct hash table or partition-then-aggregate.  `total` = records the caller is about to
 // stream in this call (the sizing of the partition regions)
 static int links_choose_mode(hh_links* lk, int64_t total) {
@@ -968,8 +991,7 @@ static int links_choose_mode(hh_links* lk, int64_t total) {
     if (lk->npart_log < 1) lk->npart_log = 1;
     if (lk->npart_log > 10) lk->npart_log = 10;
     HH_CHECK(links_new_partset(lk, total));
-    lk->spill_cap = (uint64_t)(total / 8) + (4u << 20);
-    HH_CHECK(hh_ws_alloc(lk->ctx, &lk->d_spill, (size_t)lk->spill_cap));
+    HH_CHECK(links_size_spill(lk));
     HH_CHECK(hh_dmalloc(&lk->d_spill_cursor, 1));
     HH_CUDA(cudaMemsetAsync(lk->d_spill_cursor, 0, sizeof(unsigned long long), lk->ctx->stream));
     return HH_OK;
@@ -1004,7 +1026,7 @@ static int links_part_room(hh_links* lk, int64_t n_rec) {
     if (ps.sent > 0 && ps.sent + n_rec > ps.sized_for + ps.sized_for / 8) {
         HH_CHECK(links_new_partset(lk, n_rec));
         lk->psets->back().sent = n_rec;
-        return HH_OK;
+        return links_size_spill(lk);
     }
     ps.sent += n_rec;
     return HH_OK;

@@ -1,8 +1,8 @@
-"""GPU checks at BASELINE.json's full size (configs[2]: 50k contigs / 200M pairs, the bench workload): the oracle
-cannot follow there, so the path is held to size-independent properties -- conservation of counts, key order and
-uniqueness, an independent count of the same stream with torch.unique, equality of the routed (sharded) and the
-single-table builds, stochastic columns, a valid and chromosome-pure clustering, idempotence, and equality of the
-column-sharded and the single MCL run."""
+"""GPU checks at BASELINE.json's full size (configs[2]: 50k contigs / 200M pairs, the bench workload): the link table
+bit-exact against the C oracle of the counting loop (every counter, the linked index and the matrix), plus
+size-independent properties -- conservation of counts, key order and uniqueness, equality of the routed (sharded) and
+the single-table builds, stochastic columns, a valid and chromosome-pure clustering, idempotence, and equality of the
+column-sharded and the single MCL run.  The oracle's MCL cannot follow at this size."""
 
 import numpy as np
 import pytest
@@ -31,7 +31,17 @@ def c3():
     ctx.close()
 
 
-def test_c3_link_table_properties(c3):
+@pytest.fixture(scope="module")
+def c3_oracle(c3):
+    """oracle.count_links_c of the 200M-record stream, with room for exactly the table's pairs (tens of GB of host
+    memory at this size: 64 bytes per pair inside the oracle plus its outputs)."""
+    from tests.test_gpu_links_partitioned import assert_equals_oracle
+    asm = c3["asm"]
+    return assert_equals_oracle(c3["tab"], c3["info"], c3["rec"].cpu().numpy(), asm.lengths, c3["rank"], c3["in_nx"], 500000,
+                                cap=int(c3["info"].nnz_full))
+
+
+def test_c3_link_table_properties(c3, c3_oracle):
     asm, rank, rec, tab, info = c3["asm"], c3["rank"], c3["rec"], c3["tab"], c3["info"]
     n = asm.n
     inter = rec[:, 0] != rec[:, 2]
@@ -47,18 +57,44 @@ def test_c3_link_table_properties(c3):
     assert (f["flank"] <= f["full"]).all()
     assert np.array_equal(f["ht"].astype(np.int64).sum(1), full)      # HH + HT + TH + TT = links of the pair
     assert int(tab.fetch_ctg().sum()) == 2 * int(f["flank"].astype(np.int64).sum())
-    # the same stream counted independently (torch.unique over name-ordered pair keys)
-    rk = torch.from_numpy(rank.astype(np.int64)).cuda()
-    a, b = rec[inter, 0].long(), rec[inter, 2].long()
-    swap = rk[a] > rk[b]
-    key = torch.where(swap, b, a) * n + torch.where(swap, a, b)
-    del a, b, swap
-    uniq, counts = torch.unique(key, return_counts=True)
-    del key
-    tkey = ki * n + kj
-    order = np.argsort(tkey, kind="stable")
-    assert np.array_equal(tkey[order], uniq.cpu().numpy())
-    assert np.array_equal(full[order], counts.cpu().numpy())
+    # every counter of the same stream is compared bit for bit with the C oracle by the c3_oracle fixture
+
+
+def test_c3_linked_index_and_matrix_bit_exact(c3, c3_oracle):
+    """dict_to_matrix at the bench's size: first-seen indices from the oracle's flank dict (first touch, i before j),
+    unlinked contigs after them in id order, and the symmetric matrix with self loops, bit for bit (rebuilt with torch:
+    the oracle's Python loop over tens of millions of pairs takes minutes)."""
+    asm, tab = c3["asm"], c3["tab"]
+    n = asm.n
+    keep = np.ones(n, np.uint8)
+    index, n_linked = tab.linked_index(keep)
+    tail = np.nonzero(index < 0)[0].astype(np.int32)
+    fk = torch.from_numpy(np.ascontiguousarray(c3_oracle["flank_keys"], dtype=np.int64)).cuda()
+    seq = fk.reshape(-1)                                   # i0, j0, i1, j1, ...: the touch order of dict_to_matrix (327-349)
+    big = torch.iinfo(torch.int64).max
+    touch = torch.full((n,), big, dtype=torch.int64, device=seq.device)
+    touch.scatter_reduce_(0, seq, torch.arange(len(seq), device=seq.device), "amin")
+    linked = torch.nonzero(touch < big).squeeze(1)
+    want = torch.full((n,), -1, dtype=torch.int64, device=seq.device)
+    want[linked[torch.argsort(touch[linked])]] = torch.arange(len(linked), device=seq.device)
+    assert n_linked == len(linked) and np.array_equal(index, want.cpu().numpy())
+    want[torch.from_numpy(tail.astype(np.int64)).cuda()] = torch.arange(n_linked, n, device=seq.device)
+    mat = tab.to_matrix(keep, tail)
+    got = mat.to_scipy()
+    mat.close()
+    r, c = want[fk[:, 0]], want[fk[:, 1]]
+    v = torch.from_numpy(c3_oracle["flank_vals"]).cuda().to(torch.float32)
+    diag = torch.arange(n, device=seq.device)
+    rows, cols = torch.cat([r, c, diag]), torch.cat([c, r, diag])
+    vals = torch.cat([v, v, torch.ones(n, dtype=torch.float32, device=seq.device)])
+    del fk, seq, r, c, v
+    order = torch.argsort(cols * n + rows)                  # canonical CSC; the pairs are distinct, nothing to sum
+    indptr = torch.cat([torch.zeros(1, dtype=torch.int64, device=cols.device), torch.cumsum(torch.bincount(cols, minlength=n), 0)])
+    assert np.array_equal(got.indptr, indptr.cpu().numpy())
+    assert np.array_equal(got.indices, rows[order].cpu().numpy())
+    assert np.array_equal(got.data, vals[order].cpu().numpy())
+    del touch, linked, want, rows, cols, vals, diag, order, indptr
+    torch.cuda.empty_cache()          # the library allocates outside torch's cache: leave the device memory to it
 
 
 def test_c3_routed_build_equals_single(c3):
