@@ -17,6 +17,7 @@
 #include "hh_common.cuh"
 #include "hh_internal.cuh"
 #include <stdlib.h>
+#include <algorithm>
 #include <vector>
 
 #define HH_EMPTY_KEY 0xFFFFFFFFFFFFFFFFull
@@ -80,7 +81,8 @@ struct hh_links {
     // partitioned counting (contig mode, long streams; see "partition, then aggregate" below)
     int mode;                        // 0 undecided, 1 direct (one big hash table), 2 partitioned
     int npart_log;                   // log2 of the number of partitions
-    uint64_t scap;                   // slots of a scratch table (power of two)
+    uint64_t scap;                   // slots of a shared-memory table, or of the fallback's global table when one ran
+    int64_t agg_buckets, agg_smem, agg_fallback;   // buckets at finish / counted in shared memory / by the fallback
     uint64_t spill_cap;
     std::vector<hh_partset>* psets;  // partition buffers; normally one set, a new one when a later add call outgrows it
     int4* d_spill;                   // records of partitions whose region overflowed (skewed keys), with their partition id
@@ -274,12 +276,17 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 // ---------------------------------------------------------------------------------------------
 // Partition, then aggregate.  One big hash table costs every record a random DRAM sector for the key and another
 // read-modify-write for the counters (the table is two orders of magnitude larger than L2).  For long streams the
-// records are therefore first split by the high bits of the key hash into 2^npart_log partitions (one sequential read,
-// one write in runs that fill whole sectors), and every partition is then counted in a scratch table of a few tens of
-// MB (mostly L2 hits; see links_choose_mode for its size on an H100) and emitted as compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only:
-// the result is identical to the direct path.
+// records are therefore split twice by the high bits of the key hash: into 2^npart_log partition regions while they
+// stream in, and at finish into 2^bucket_log buckets (the next hash bits, links_bucket_log) laid out densely.  A bucket
+// (about 1.3k records at the benchmark's 200M records) is then counted in an open-addressing table in shared memory and emitted as
+// compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only: the result is identical to
+// the direct path.
 //   hh_k_part_scatter   record -> {i, j, stream index, flags} (ends ordered by name rank, is_flank / head-tail evaluated once)
-//   hh_k_part_step      emit + clear the scratch table of the previous partition, count the current one into the other
+//   hh_k_part_hist      records per bucket (shared-memory histogram of a region's sub-buckets per tile)
+//   hh_k_part_scatter2  the same pass again: every record to its place in the dense bucket buffer
+//   hh_k_bucket_count   persistent CTAs: count one bucket at a time in shared memory, emit its live slots, clear
+//   hh_k_part_step      fallback for the buckets a shared-memory table cannot take: gathered, then counted in batches of
+//                       about 2^19 records through global scratch tables
 // ---------------------------------------------------------------------------------------------
 #define HH_PART_TILE 4096          // records per tile of the scatter kernel (512 threads x 8)
 #define HH_PART_MAX 1024
@@ -354,19 +361,314 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
     if (threadIdx.x == 0 && s_used) atomicAdd(counters + 1, (unsigned long long)s_used);
 }
 
-// count `n` partitioned records ({i, j, stream index, flags}) into a scratch table; part >= 0 selects the records of
-// that partition from a mixed list (the spill list)
-__device__ __forceinline__ void hh_part_count(const int4* __restrict__ prec, int64_t n, int part, uint64_t* __restrict__ keys,
+// ---- level 2: buckets -------------------------------------------------------------------------------------------------
+// A bucket is the top bucket_log bits of hh_mix64(key): the partition (top npart_log bits) and below it a sub-bucket.
+#define HH_AGG_MEAN 2048           // buckets hold at most this many records on average (links_bucket_log)
+#define HH_SUB_MAX_LOG 12          // at most 2^12 sub-buckets per partition region: the shared histograms of hist / scatter2
+#define HH_AGG_SLOTS 2048          // slots of a shared-memory table (36 B each: 72 KiB, three CTAs per SM)
+#define HH_AGG_THREADS 256
+#define HH_AGG_HOT 32              // a bucket with more than HH_AGG_HOT x the mean records skips shared memory (links_hot_records)
+
+__device__ __forceinline__ uint32_t hh_bucket_of(int4 r, int bucket_log) {
+    const uint64_t key = ((uint64_t)(uint32_t)r.x << 32) | (uint64_t)(uint32_t)r.y;
+    return (uint32_t)(hh_mix64(key) >> (64 - bucket_log));
+}
+
+// Records per bucket.  The virtual tiles are `tpr` tiles of every region (those past the region's fill exit at once),
+// then the spill list; a region tile histograms its 2^(bucket_log - npart_log) sub-buckets in shared memory and adds them
+// with one global atomic per sub-bucket.  Spill records (rare) go straight to their bucket.
+__global__ void __launch_bounds__(512)
+hh_k_part_hist(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int64_t tpr,
+               const int4* __restrict__ spill, int64_t n_spill, int bucket_log, unsigned int* __restrict__ bcnt) {
+    __shared__ unsigned int s_cnt[1 << HH_SUB_MAX_LOG];
+    const int sub_log = bucket_log - npart_log, nsub = 1 << sub_log;
+    const int64_t region_tiles = ((int64_t)1 << npart_log) * tpr;
+    const int64_t tiles = region_tiles + (n_spill + HH_PART_TILE - 1) / HH_PART_TILE;
+    for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+        if (t >= region_tiles) {
+            const int64_t base = (t - region_tiles) * HH_PART_TILE;
+            for (int k = threadIdx.x; k < HH_PART_TILE; k += 512)
+                if (base + k < n_spill) atomicAdd(bcnt + hh_bucket_of(hh_ld_stream(spill + base + k), bucket_log), 1u);
+            continue;
+        }
+        const int p = (int)(t / tpr);
+        const uint64_t start = (uint64_t)(t % tpr) * HH_PART_TILE;
+        const uint64_t fill = min((uint64_t)cursor[p], pcap);
+        if (start >= fill) continue;                    // block-uniform
+        for (int k = threadIdx.x; k < nsub; k += 512) s_cnt[k] = 0;
+        __syncthreads();
+        const int4* reg = pbuf + (size_t)p * (size_t)pcap;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const uint64_t i = start + (uint64_t)k * 512 + threadIdx.x;
+            if (i < fill) atomicAdd(&s_cnt[hh_bucket_of(hh_ld_stream(reg + i), bucket_log) & (nsub - 1)], 1u);
+        }
+        __syncthreads();
+        for (int k = threadIdx.x; k < nsub; k += 512)
+            if (s_cnt[k]) atomicAdd(bcnt + ((size_t)p << sub_log) + k, s_cnt[k]);
+        __syncthreads();
+    }
+}
+
+// The pass of hh_k_part_hist again: every record goes to boff[bucket] + its rank.  Ranks inside a tile come from shared
+// memory, one global atomic per (tile, sub-bucket) reserves the tile's run; bfill counts what each bucket received.
+__global__ void __launch_bounds__(512, 2)
+hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int64_t tpr,
+                   const int4* __restrict__ spill, int64_t n_spill, int bucket_log, const int64_t* __restrict__ boff,
+                   unsigned int* __restrict__ bfill, int4* __restrict__ out, uint64_t n_out, unsigned long long* __restrict__ counters) {
+    __shared__ unsigned int s_cnt[1 << HH_SUB_MAX_LOG];
+    __shared__ unsigned int s_base[1 << HH_SUB_MAX_LOG];
+    const int sub_log = bucket_log - npart_log, nsub = 1 << sub_log;
+    const int64_t region_tiles = ((int64_t)1 << npart_log) * tpr;
+    const int64_t tiles = region_tiles + (n_spill + HH_PART_TILE - 1) / HH_PART_TILE;
+    for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+        if (t >= region_tiles) {
+            const int64_t base = (t - region_tiles) * HH_PART_TILE;
+            for (int k = threadIdx.x; k < HH_PART_TILE; k += 512) {
+                if (base + k >= n_spill) break;
+                const int4 r = hh_ld_stream(spill + base + k);
+                const uint32_t b = hh_bucket_of(r, bucket_log);
+                const uint64_t q = (uint64_t)boff[b] + atomicAdd(bfill + b, 1u);
+                if (q < n_out) out[q] = r;
+                else atomicExch(counters + 2, 6ull);
+            }
+            continue;
+        }
+        const int p = (int)(t / tpr);
+        const uint64_t start = (uint64_t)(t % tpr) * HH_PART_TILE;
+        const uint64_t fill = min((uint64_t)cursor[p], pcap);
+        if (start >= fill) continue;                    // block-uniform
+        for (int k = threadIdx.x; k < nsub; k += 512) s_cnt[k] = 0;
+        __syncthreads();
+        const int4* reg = pbuf + (size_t)p * (size_t)pcap;
+        int4 r[8];
+        uint32_t at[8];                                 // sub-bucket << 16 | rank in the tile (both < 2^13), ~0 = none
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const uint64_t i = start + (uint64_t)k * 512 + threadIdx.x;
+            at[k] = HH_NONE32;
+            if (i < fill) {
+                r[k] = hh_ld_stream(reg + i);
+                const uint32_t sub = hh_bucket_of(r[k], bucket_log) & (nsub - 1);
+                at[k] = (sub << 16) | atomicAdd(&s_cnt[sub], 1u);
+            }
+        }
+        __syncthreads();
+        for (int k = threadIdx.x; k < nsub; k += 512)
+            if (s_cnt[k]) s_base[k] = atomicAdd(bfill + ((size_t)p << sub_log) + k, s_cnt[k]);
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            if (at[k] == HH_NONE32) continue;
+            const uint32_t sub = at[k] >> 16;
+            const size_t b = ((size_t)p << sub_log) + sub;
+            const uint64_t q = (uint64_t)boff[b] + s_base[sub] + (at[k] & 0xFFFFu);
+            if (q < n_out) out[q] = r[k];
+            else atomicExch(counters + 2, 6ull);
+        }
+        __syncthreads();
+    }
+}
+
+// Count every bucket in shared memory.  Persistent CTAs take buckets from an atomic queue (agg[0]).  A bucket's table is
+// the power of two >= 1.5 x its records (at least one slot per thread, at most HH_AGG_SLOTS), stored SoA: u64 keys and
+// the seven u32 counters of hh_slot.  Nothing leaves the CTA before the bucket has counted completely: a bucket whose
+// distinct keys exceed 3/4 of the table (or whose probe finds no slot) is abandoned -- its table is cleared and it goes
+// on the fallback list (agg[1] entries), as does a bucket of more than `hot` records.  A completed bucket is emitted
+// (one global atomic reserves its entries, a block scan per 256 slots ranks them, so a warp writes consecutive entries),
+// with the per-fragment totals and nnz_flank, and only the slots it used are cleared.  agg[2] counts completed buckets.
+__global__ void __launch_bounds__(HH_AGG_THREADS, 3)
+hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff, int nbuckets, uint64_t hot,
+                  uint32_t* __restrict__ compact, uint64_t compact_cap, unsigned long long* __restrict__ ctg_links,
+                  unsigned long long* __restrict__ counters, unsigned long long* __restrict__ agg, uint32_t* __restrict__ fallback) {
+    extern __shared__ __align__(16) unsigned char hh_agg_smem[];
+    uint64_t* tkey = reinterpret_cast<uint64_t*>(hh_agg_smem);
+    uint32_t* t_full = reinterpret_cast<uint32_t*>(tkey + HH_AGG_SLOTS);
+    uint32_t* t_flank = t_full + HH_AGG_SLOTS;
+    uint32_t* t_ffull = t_flank + HH_AGG_SLOTS;
+    uint32_t* t_fflank = t_ffull + HH_AGG_SLOTS;
+    uint32_t* t_ht = t_fflank + HH_AGG_SLOTS;
+    uint32_t* t_th = t_ht + HH_AGG_SLOTS;
+    uint32_t* t_tt = t_th + HH_AGG_SLOTS;
+    __shared__ int s_bucket;
+    __shared__ unsigned int s_distinct, s_abandon;
+    __shared__ unsigned int s_wtot[HH_AGG_THREADS / 32];
+    __shared__ unsigned long long s_base;
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    auto clear = [&](int s) {
+        tkey[s] = HH_EMPTY_KEY;
+        t_full[s] = 0u;
+        t_flank[s] = 0u;
+        t_ffull[s] = HH_NONE32;
+        t_fflank[s] = HH_NONE32;
+        t_ht[s] = 0u;
+        t_th[s] = 0u;
+        t_tt[s] = 0u;
+    };
+    for (int s = threadIdx.x; s < HH_AGG_SLOTS; s += HH_AGG_THREADS) clear(s);
+    unsigned int nfl = 0, n_done = 0;
+    for (;;) {
+        __syncthreads();                            // the previous bucket is finished with every shared variable
+        if (threadIdx.x == 0) {
+            s_bucket = (int)atomicAdd(agg + 0, 1ull);
+            s_distinct = 0;
+            s_abandon = 0;
+        }
+        __syncthreads();
+        const int bk = s_bucket;
+        if (bk >= nbuckets) break;
+        const int64_t lo = boff[bk], n = boff[bk + 1] - lo;
+        if ((uint64_t)n > hot) {
+            if (threadIdx.x == 0) fallback[atomicAdd(agg + 1, 1ull)] = (uint32_t)bk;
+            continue;
+        }
+        int tsize = HH_AGG_THREADS;
+        while (tsize < HH_AGG_SLOTS && (int64_t)tsize * 2 < n * 3) tsize <<= 1;
+        const unsigned int limit = (unsigned)tsize / 4 * 3;
+        const unsigned int mask = (unsigned)tsize - 1;
+        // ---- count
+        for (int64_t i0 = (int64_t)wv * 32; i0 < n; i0 += HH_AGG_THREADS) {
+            const int64_t i = i0 + lane;
+            const bool ok = i < n;
+            int4 r = make_int4(0, 0, 0, 0);
+            if (ok) r = hh_ld_stream(rec + lo + i);
+            const unsigned f = (unsigned)r.w;
+            const uint64_t key = ok ? (((uint64_t)(uint32_t)r.x << 32) | (uint64_t)(uint32_t)r.y) : (HH_EMPTY_KEY - 1 - (uint64_t)lane);
+            const unsigned peers = __match_any_sync(HH_FULL_MASK, key);
+            const bool fl = ok && (f & 1u), ti = (f & 2u) != 0, tj = (f & 4u) != 0;
+            const uint32_t idx = ok ? (uint32_t)r.z : HH_NONE32;
+            const uint32_t first_all = __reduce_min_sync(peers, idx);
+            const uint32_t first_fl = __reduce_min_sync(peers, fl ? idx : HH_NONE32);
+            const unsigned b_fl = __ballot_sync(HH_FULL_MASK, fl);
+            const unsigned b_ht = __ballot_sync(HH_FULL_MASK, ok && !ti && tj);
+            const unsigned b_th = __ballot_sync(HH_FULL_MASK, ok && ti && !tj);
+            const unsigned b_tt = __ballot_sync(HH_FULL_MASK, ok && ti && tj);
+            if (ok && lane == (__ffs(peers) - 1)) {
+                unsigned int slot = (unsigned int)hh_mix64(key) & mask;
+                int probes = 0;
+                for (; probes < tsize; ++probes) {
+                    const uint64_t k = *((volatile uint64_t*)(tkey + slot));
+                    if (k == key) break;
+                    if (k == HH_EMPTY_KEY) {
+                        const unsigned long long prev = atomicCAS((unsigned long long*)(tkey + slot), (unsigned long long)HH_EMPTY_KEY,
+                                                                  (unsigned long long)key);
+                        if (prev == HH_EMPTY_KEY) {
+                            if (atomicAdd(&s_distinct, 1u) >= limit) s_abandon = 1;
+                            break;
+                        }
+                        if (prev == key) break;
+                    }
+                    slot = (slot + 1) & mask;
+                }
+                if (probes == tsize) {
+                    s_abandon = 1;
+                } else {
+                    atomicAdd(t_full + slot, (unsigned)__popc(peers));
+                    atomicMin(t_ffull + slot, first_all);
+                    const unsigned c_fl = __popc(peers & b_fl);
+                    if (c_fl) {
+                        atomicAdd(t_flank + slot, c_fl);
+                        atomicMin(t_fflank + slot, first_fl);
+                    }
+                    const unsigned c_ht = __popc(peers & b_ht), c_th = __popc(peers & b_th), c_tt = __popc(peers & b_tt);
+                    if (c_ht) atomicAdd(t_ht + slot, c_ht);
+                    if (c_th) atomicAdd(t_th + slot, c_th);
+                    if (c_tt) atomicAdd(t_tt + slot, c_tt);
+                }
+            }
+            if (__any_sync(HH_FULL_MASK, *((volatile unsigned int*)&s_abandon) != 0)) break;
+        }
+        __syncthreads();
+        if (s_abandon) {
+            for (int s = threadIdx.x; s < tsize; s += HH_AGG_THREADS) clear(s);
+            if (threadIdx.x == 0) fallback[atomicAdd(agg + 1, 1ull)] = (uint32_t)bk;
+            continue;
+        }
+        // ---- emit + clear
+        if (threadIdx.x == 0) s_base = s_distinct ? atomicAdd(counters + 0, (unsigned long long)s_distinct) : 0ull;
+        __syncthreads();
+        unsigned long long run = s_base;
+        for (int s0 = 0; s0 < tsize; s0 += HH_AGG_THREADS) {
+            const int s = s0 + threadIdx.x;
+            const uint64_t key = tkey[s];
+            const bool live = key != HH_EMPTY_KEY;
+            const unsigned bal = __ballot_sync(HH_FULL_MASK, live);
+            if (lane == 0) s_wtot[wv] = __popc(bal);
+            __syncthreads();
+            unsigned int before = 0, total = 0;
+#pragma unroll
+            for (int k = 0; k < HH_AGG_THREADS / 32; ++k) {
+                const unsigned int t = s_wtot[k];
+                before += (k < wv) ? t : 0u;
+                total += t;
+            }
+            if (live) {
+                const unsigned long long pos = run + before + __popc(bal & ((1u << lane) - 1u));
+                const uint32_t flank = t_flank[s];
+                if (pos < compact_cap) {
+                    uint32_t* o = compact + pos * 9;
+                    o[0] = (uint32_t)(key >> 32);
+                    o[1] = (uint32_t)key;
+                    o[2] = t_full[s];
+                    o[3] = flank;
+                    o[4] = t_ffull[s];
+                    o[5] = t_fflank[s];
+                    o[6] = t_ht[s];
+                    o[7] = t_th[s];
+                    o[8] = t_tt[s];
+                } else {
+                    atomicExch(counters + 2, 5ull);
+                }
+                if (flank) {
+                    nfl++;
+                    atomicAdd(ctg_links + (uint32_t)(key >> 32), (unsigned long long)flank);      // ctg_link_dict (1638-1639)
+                    atomicAdd(ctg_links + (uint32_t)key, (unsigned long long)flank);
+                }
+                clear(s);
+            }
+            run += total;
+            __syncthreads();                        // s_wtot is rewritten by the next trip
+        }
+        n_done++;
+    }
+    nfl = (unsigned)hh_warp_sum((int)nfl);
+    if (lane == 0 && nfl) atomicAdd(counters + 3, (unsigned long long)nfl);
+    if (threadIdx.x == 0 && n_done) atomicAdd(agg + 2, (unsigned long long)n_done);
+}
+
+// ---- fallback: the global scratch table ------------------------------------------------------------------------------
+// The listed buckets are gathered into one dense list and counted in batches of about HH_FB_BATCH records, so that the
+// number of launches grows with the records that fall back and not with the buckets.  Buckets are functions of the key,
+// so the keys of different buckets never meet and a batch may hold any number of them.
+#define HH_FB_BATCH (1 << 19)      // records per fallback batch: two 2^20-slot scratch tables of 42 MB at load <= 0.5
+
+// dst[pre[k] + r] = src[src_off[k] + r] for the nf listed buckets (pre = exclusive prefix of their record counts)
+__global__ void hh_k_gather_buckets(const int4* __restrict__ src, const int64_t* __restrict__ src_off, const int64_t* __restrict__ pre,
+                                    int nf, int4* __restrict__ dst) {
+    const int64_t total = pre[nf];
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        int lo = 0, hi = nf - 1;                   // the last bucket that starts at or before i
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (pre[mid] <= i) lo = mid;
+            else hi = mid - 1;
+        }
+        dst[i] = hh_ld_stream(src + src_off[lo] + (i - pre[lo]));
+    }
+}
+
+// count `n` bucket records ({i, j, stream index, flags}) into a scratch table
+__device__ __forceinline__ void hh_part_count(const int4* __restrict__ prec, int64_t n, uint64_t* __restrict__ keys,
                                               hh_slot* __restrict__ vals, uint64_t cap, unsigned long long* __restrict__ counters) {
     const int lane = threadIdx.x & 31;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x - lane); i0 < n; i0 += stride) {
         const int64_t i = i0 + lane;
-        bool ok = i < n;
+        const bool ok = i < n;
         int4 r = make_int4(0, 0, 0, 0);
         if (ok) r = hh_ld_stream(prec + i);
         const unsigned f = (unsigned)r.w;
-        if (ok && part >= 0) ok = (int)(f >> 8) == part;
         const uint64_t key = ok ? (((uint64_t)(uint32_t)r.x << 32) | (uint64_t)(uint32_t)r.y) : (HH_EMPTY_KEY - 1 - (uint64_t)lane);
         const unsigned peers = __match_any_sync(HH_FULL_MASK, key);
         const bool fl = ok && (f & 1u), ti = (f & 2u) != 0, tj = (f & 4u) != 0;
@@ -391,12 +693,12 @@ __device__ __forceinline__ void hh_part_count(const int4* __restrict__ prec, int
     }
 }
 
+// count one bucket into the scratch table (ckeys), or emit the table (ekeys)
 __global__ void __launch_bounds__(256)
-hh_k_part_step(const int4* __restrict__ prec, int64_t n, const int4* __restrict__ spill, int64_t n_spill, int part,
-               uint64_t* __restrict__ ckeys, hh_slot* __restrict__ cvals, uint64_t* __restrict__ ekeys, hh_slot* __restrict__ evals, uint64_t cap,
-               uint32_t* __restrict__ compact, uint64_t compact_cap, unsigned long long* __restrict__ ctg_links,
-               unsigned long long* __restrict__ counters) {
-    // ---- emit the table of the previous partition: live slots -> compact entries, per-fragment totals; slots are cleared.
+hh_k_part_step(const int4* __restrict__ prec, int64_t n, uint64_t* __restrict__ ckeys, hh_slot* __restrict__ cvals,
+               uint64_t* __restrict__ ekeys, hh_slot* __restrict__ evals, uint64_t cap, uint32_t* __restrict__ compact,
+               uint64_t compact_cap, unsigned long long* __restrict__ ctg_links, unsigned long long* __restrict__ counters) {
+    // ---- emit the table of the previous bucket: live slots -> compact entries, per-fragment totals; slots are cleared.
     // A CTA takes 512 consecutive slots, two per thread: the keys are loaded together (one memory round trip instead
     // of one per slot), the live ones are ranked by a block scan, the output positions of the whole CTA are reserved with
     // ONE atomic on the global cursor, then the values are read together and written.
@@ -478,11 +780,8 @@ hh_k_part_step(const int4* __restrict__ prec, int64_t n, const int4* __restrict_
         nfl = (unsigned)hh_warp_sum((int)nfl);
         if (lane == 0 && nfl) atomicAdd(counters + 3, (unsigned long long)nfl);
     }
-    // ---- count the current partition
-    if (ckeys != nullptr) {
-        if (n > 0) hh_part_count(prec, n, -1, ckeys, cvals, cap, counters);
-        if (n_spill > 0) hh_part_count(spill, n_spill, part, ckeys, cvals, cap, counters);
-    }
+    // ---- count the current bucket
+    if (ckeys != nullptr && n > 0) hh_part_count(prec, n, ckeys, cvals, cap, counters);
 }
 
 // re-insert every live slot of the old table into a (larger) new one
@@ -983,9 +1282,7 @@ static int links_choose_mode(hh_links* lk, int64_t total) {
     }
     lk->mode = 2;
     int lg = 4;
-    // ~400k records per partition, at most 512 partitions.  At 200M records the two scratch tables (2 x 2^20 slots, 42 MB
-    // each) exceed the H100's 50 MB L2; 1024 partitions (2 x 21 MB, inside L2) were measured slower on an H100 SXM:
-    // link build 46.3 ms against 42.4-42.8 ms -- a step is a latency chain, not bound by where the table lives
+    // ~400k records per partition, at most 512 partitions (the buckets of links_bucket_log split them further at finish)
     while (lg < 9 && ((int64_t)400000 << lg) < total) lg++;
     lk->npart_log = links_env_int("HH_LINKS_NPART_LOG", lg);
     if (lk->npart_log < 1) lk->npart_log = 1;
@@ -1099,8 +1396,9 @@ extern "C" int hh_links_add(hh_links* lk, const int32_t* rec, int64_t n_rec, int
     return HH_OK;
 }
 
-// partitioned counting, second phase: every partition through a small scratch table (two tables, so the emit of
-// partition p - 1 and the count of partition p share one launch), entries appended to an unordered compact list
+// partitioned counting, second phase (see "partition, then aggregate"): the regions are split into dense buckets, every
+// bucket is counted in shared memory and the few that a shared-memory table cannot take in a global scratch table;
+// entries are appended to an unordered compact list
 static void links_free_partsets(hh_links* lk) {
     if (lk->psets) {
         for (size_t k = 0; k < lk->psets->size(); ++k) {
@@ -1113,9 +1411,33 @@ static void links_free_partsets(hh_links* lk) {
     hh_dfree(lk->d_spill_cursor);
 }
 
+// log2 of the number of buckets for n_used records: a mean of at most HH_AGG_MEAN records per bucket (200M records:
+// 2^17 buckets of about 1.3k records, 256 per partition), at least one bucket per partition region, at most
+// 2^HH_SUB_MAX_LOG per region
+static int links_bucket_log(int64_t n_used, int npart_log) {
+    int b = npart_log;
+    while (b < npart_log + HH_SUB_MAX_LOG && (n_used >> b) > HH_AGG_MEAN) b++;
+    return b;
+}
+
+// records above which a bucket goes to the fallback without trying shared memory: HH_AGG_HOT x the mean bucket, and at
+// least HH_AGG_HOT x HH_AGG_MEAN / 2.  Counting a bucket costs about its records, and a CTA of hh_k_bucket_count takes
+// about buckets / (3 x SMs) of them (about 330 at 200M records on an H100), so a bucket at the threshold is a tenth of a
+// CTA's share.  A hot contig pair above it would make one CTA a straggler; the fallback spreads it over the whole GPU.
+static uint64_t links_hot_records(int64_t n_used, int bucket_log) {
+    const uint64_t mean = ((uint64_t)n_used + (1ull << bucket_log) - 1) >> bucket_log;
+    return (uint64_t)HH_AGG_HOT * (mean > HH_AGG_MEAN / 2 ? mean : HH_AGG_MEAN / 2);
+}
+
+// Device memory of the finish for P records sent, U of them usable: the regions (24 B x P + 32 MB at 512 partitions) and
+// the spill list (2 B x P + 64 MB), the bucket buffer (16 B x U) and the compact staging list (36 B x U).  The regions and
+// the spill list are released before the staging list is allocated, so at most 8.7 GB is in use at once at the
+// benchmark's 200M records (U = 167M).  Released blocks stay in the context's workspace cache, which gives them back only
+// when an allocation fails, and the staging list does not fit the regions' block: the process holds all four, 14.0 GB,
+// where the partition step this replaced held 11.4 GB (regions, spill list, staging list, two 42 MB scratch tables).  A
+// fallback adds its gathered records (16 B each), which take the place of the bucket buffer, and two scratch tables.
 static int links_finish_partitioned(hh_links* lk) {
     hh_ctx* ctx = lk->ctx;
-    const int npart = 1 << lk->npart_log;
     const size_t nsets = lk->psets->size();
     unsigned long long c[8];
     HH_CHECK(links_read_counters(lk, c));
@@ -1123,59 +1445,114 @@ static int links_finish_partitioned(hh_links* lk) {
                "hh_links_finish: the spill list of the partitioned counting overflowed (a few contig pairs own most of the stream): "
                "set HH_LINKS_PARTITION=0 to use the direct hash table");
     lk->n_used = lk->peer_used + (int64_t)c[1];
-    // region fill levels and the spill count
-    std::vector<unsigned long long> fill(nsets * (size_t)npart);
-    for (size_t k = 0; k < nsets; ++k)
-        HH_CUDA(cudaMemcpyAsync(fill.data() + k * (size_t)npart, (*lk->psets)[k].cursor, (size_t)npart * sizeof(unsigned long long),
-                                cudaMemcpyDeviceToHost, ctx->stream));
+    const int64_t U = (int64_t)c[1];                       // records in the regions and on the spill list
+    HH_REQUIRE(U < (1ll << 31), HH_ERR_UNSUPPORTED,
+               "hh_links_finish: %lld usable records; the partitioned counting takes fewer than 2^31: set HH_LINKS_PARTITION=0",
+               (long long)U);
     unsigned long long n_spill = 0;
     HH_CUDA(cudaMemcpyAsync(&n_spill, lk->d_spill_cursor, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
     HH_CUDA(cudaStreamSynchronize(ctx->stream));
-    // scratch tables: load factor <= 0.6 even if every record of the fullest partition is a distinct key
-    unsigned long long worst = 1;
-    for (int p = 0; p < npart; ++p) {
-        unsigned long long t = 0;
-        for (size_t k = 0; k < nsets; ++k) t += fill[k * (size_t)npart + p];
-        if (t > worst) worst = t;
-    }
-    uint64_t scap = 1ull << 12;
-    while ((double)scap * 0.6 < (double)worst) scap <<= 1;
-    lk->scap = scap;
+    const int blog = links_bucket_log(U, lk->npart_log);
+    const int nb = 1 << blog;
+    const uint64_t hot = links_hot_records(U, blog);
+    const uint64_t compact_cap = (uint64_t)(U > 0 ? U : 1);       // distinct pairs <= usable records
+    unsigned int *d_bcnt = nullptr, *d_bfill = nullptr;
+    uint32_t *d_fallback = nullptr, *d_stage_compact = nullptr;  // the exact-size list is cut from the staging list
+    int64_t* d_boff = nullptr;
+    unsigned long long* d_agg = nullptr;
+    int4 *d_rec2 = nullptr, *d_fb_rec = nullptr;
+    int64_t* d_fb_off = nullptr;                                  // fallback: [nf] bucket offsets, [nf + 1] prefix of their records
     uint64_t* skeys[2] = {nullptr, nullptr};
     hh_slot* svals[2] = {nullptr, nullptr};
-    const uint64_t compact_cap = (uint64_t)(lk->n_used > 0 ? lk->n_used : 1);       // distinct pairs <= usable records
     hh_dfree(lk->d_compact);
-    uint32_t* d_stage_compact = nullptr;                                              // workspace; the exact-size list is cut from it
     int rc = [&]() -> int {
+        HH_CHECK(hh_dmalloc(&d_bcnt, (size_t)nb));
+        HH_CHECK(hh_dmalloc(&d_bfill, (size_t)nb));
+        HH_CHECK(hh_dmalloc(&d_boff, (size_t)nb + 1));
+        HH_CHECK(hh_dmalloc(&d_fallback, (size_t)nb));
+        HH_CHECK(hh_dmalloc(&d_agg, 4));
+        HH_CHECK(hh_ws_alloc(ctx, &d_rec2, (size_t)compact_cap));
+        HH_CUDA(cudaMemsetAsync(d_bcnt, 0, (size_t)nb * sizeof(unsigned int), ctx->stream));
+        HH_CUDA(cudaMemsetAsync(d_bfill, 0, (size_t)nb * sizeof(unsigned int), ctx->stream));
+        HH_CUDA(cudaMemsetAsync(d_agg, 0, 4 * sizeof(unsigned long long), ctx->stream));
+        // ---- buckets: records per bucket, dense offsets, every record to its bucket
+        const int grid = hh_grid(ctx, 4);
+        for (size_t k = 0; k < nsets; ++k) {
+            const hh_partset& ps = (*lk->psets)[k];
+            const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
+            HH_LAUNCH(ctx, hh_k_part_hist, grid, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
+                      k == 0 ? (int64_t)n_spill : 0, blog, d_bcnt);
+        }
+        HH_CHECK(hh_exclusive_scan_i32(ctx, reinterpret_cast<const int*>(d_bcnt), d_boff, nb));
+        for (size_t k = 0; k < nsets; ++k) {
+            const hh_partset& ps = (*lk->psets)[k];
+            const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
+            HH_LAUNCH(ctx, hh_k_part_scatter2, grid, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
+                      k == 0 ? (int64_t)n_spill : 0, blog, d_boff, d_bfill, d_rec2, compact_cap, lk->d_counters);
+        }
+        links_free_partsets(lk);                               // ordered on the stream behind scatter2
         HH_CHECK(hh_ws_alloc(ctx, &d_stage_compact, (size_t)compact_cap * 9));
-        for (int b = 0; b < 2; ++b) HH_CHECK(links_alloc_table(lk, scap, &skeys[b], &svals[b]));
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 0, 0, sizeof(unsigned long long), ctx->stream));     // entry cursor
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));     // nnz_flank
-        const int grid = hh_grid(ctx, 8);
-        for (int p = 0; p <= npart; ++p) {
-            const int cb = p & 1, eb = cb ^ 1;
-            bool first = true;
-            for (size_t k = 0; k < nsets || first; ++k) {
-                const bool have = p < npart && k < nsets;
-                const uint64_t pcap = k < nsets ? (*lk->psets)[k].pcap : 0;
-                unsigned long long nrec = have ? fill[k * (size_t)npart + p] : 0;
-                if (have && nrec > pcap) nrec = pcap;                 // the excess is on the spill list
-                const int4* prec = have ? (*lk->psets)[k].buf + (size_t)p * (size_t)pcap : nullptr;
-                // the spill list is scanned once per overflowed partition (with the first set)
-                bool spill_now = false;
-                if (p < npart && first && n_spill) {
-                    for (size_t kk = 0; kk < nsets; ++kk) spill_now = spill_now || fill[kk * (size_t)npart + p] > (*lk->psets)[kk].pcap;
-                }
-                HH_LAUNCH(ctx, hh_k_part_step, grid, 256, 0, prec, (int64_t)nrec, lk->d_spill, spill_now ? (int64_t)n_spill : 0, p,
-                          p < npart ? skeys[cb] : nullptr, p < npart ? svals[cb] : nullptr, (first && p > 0) ? skeys[eb] : nullptr,
-                          (first && p > 0) ? svals[eb] : nullptr, scap, d_stage_compact, compact_cap, lk->d_ctg, lk->d_counters);
-                first = false;
-                if (k + 1 >= nsets) break;
-            }
-        }
+        // ---- every bucket in shared memory
+        const size_t smem = (size_t)HH_AGG_SLOTS * (sizeof(uint64_t) + 7 * sizeof(uint32_t));
+        HH_CUDA(cudaFuncSetAttribute(hh_k_bucket_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int per_sm = 0;
+        HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hh_k_bucket_count, HH_AGG_THREADS, smem));
+        HH_REQUIRE(per_sm > 0, HH_ERR_CUDA, "hh_links_finish: the bucket counting kernel does not fit an SM");
+        HH_LAUNCH(ctx, hh_k_bucket_count, hh_grid(ctx, per_sm), HH_AGG_THREADS, smem, d_rec2, d_boff, nb, hot, d_stage_compact,
+                  compact_cap, lk->d_ctg, lk->d_counters, d_agg, d_fallback);
+        unsigned long long agg[4];
+        HH_CUDA(cudaMemcpyAsync(agg, d_agg, sizeof(agg), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CHECK(links_read_counters(lk, c));
+        lk->agg_buckets = nb;
+        lk->agg_smem = (int64_t)agg[2];
+        lk->agg_fallback = (int64_t)agg[1];
+        lk->scap = HH_AGG_SLOTS;
+        // ---- fallback: the listed buckets' records are gathered into one list and counted in batches through two global
+        // scratch tables (load <= 0.6 even if every record of the largest batch is a distinct key): launch t emits +
+        // clears the table of batch t - 1 and counts batch t into the other
+        if (agg[1]) {
+            const int nf = (int)agg[1];
+            std::vector<uint32_t> fb((size_t)nf);
+            std::vector<int64_t> off((size_t)nb + 1), src_off((size_t)nf), pre((size_t)nf + 1, 0);
+            HH_CUDA(cudaMemcpyAsync(fb.data(), d_fallback, fb.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+            HH_CUDA(cudaMemcpyAsync(off.data(), d_boff, off.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+            HH_CUDA(cudaStreamSynchronize(ctx->stream));
+            std::vector<int64_t> cut(1, 0);                    // batch t = gathered records [cut[t], cut[t + 1])
+            for (int k = 0; k < nf; ++k) {
+                src_off[k] = off[fb[k]];
+                const int64_t n = off[fb[k] + 1] - off[fb[k]];
+                if (pre[k] > cut.back() && pre[k] + n - cut.back() > HH_FB_BATCH) cut.push_back(pre[k]);
+                pre[k + 1] = pre[k] + n;
+            }
+            cut.push_back(pre[nf]);
+            int64_t worst = 1;
+            for (size_t t = 0; t + 1 < cut.size(); ++t) worst = std::max(worst, cut[t + 1] - cut[t]);
+            uint64_t scap = 1ull << 12;
+            while ((double)scap * 0.6 < (double)worst) scap <<= 1;
+            lk->scap = scap;
+            HH_CHECK(hh_dmalloc(&d_fb_off, 2 * (size_t)nf + 1));
+            HH_CUDA(cudaMemcpyAsync(d_fb_off, src_off.data(), (size_t)nf * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
+            HH_CUDA(cudaMemcpyAsync(d_fb_off + nf, pre.data(), ((size_t)nf + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
+            HH_CHECK(hh_ws_alloc(ctx, &d_fb_rec, (size_t)pre[nf]));
+            HH_LAUNCH(ctx, hh_k_gather_buckets, hh_grid(ctx, 8), 256, 0, d_rec2, d_fb_off, d_fb_off + nf, nf, d_fb_rec);
+            hh_ws_free(ctx, d_rec2);                           // ordered on the stream behind the gather
+            for (int t = 0; t < 2; ++t) HH_CHECK(links_alloc_table(lk, scap, &skeys[t], &svals[t]));
+            const int g = hh_grid(ctx, 8);
+            const int nbatch = (int)cut.size() - 1;
+            for (int t = 0; t <= nbatch; ++t) {
+                const int cb = t & 1, eb = cb ^ 1;
+                const bool have = t < nbatch;
+                HH_LAUNCH(ctx, hh_k_part_step, g, 256, 0, have ? d_fb_rec + cut[t] : (const int4*)nullptr,
+                          have ? cut[t + 1] - cut[t] : (int64_t)0, have ? skeys[cb] : (uint64_t*)nullptr,
+                          have ? svals[cb] : (hh_slot*)nullptr, t > 0 ? skeys[eb] : (uint64_t*)nullptr,
+                          t > 0 ? svals[eb] : (hh_slot*)nullptr, scap, d_stage_compact, compact_cap, lk->d_ctg, lk->d_counters);
+            }
+            HH_CHECK(links_read_counters(lk, c));
+        }
         HH_REQUIRE(c[2] == 0, HH_ERR_CAPACITY,
-                   "hh_links_finish: a scratch table of the partitioned counting overflowed (code %llu): set HH_LINKS_PARTITION=0", c[2]);
+                   "hh_links_finish: a bucket of the partitioned counting overflowed (code %llu): set HH_LINKS_PARTITION=0", c[2]);
         lk->nnz = (int64_t)c[0];
         lk->nnz_flank = (int64_t)c[3];
         HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(lk->nnz > 0 ? lk->nnz : 1) * 9));
@@ -1185,14 +1562,30 @@ static int links_finish_partitioned(hh_links* lk) {
         return HH_OK;
     }();
     hh_ws_free(ctx, d_stage_compact);
-    for (int b = 0; b < 2; ++b) {
-        hh_dfree(skeys[b]);
-        hh_dfree(svals[b]);
+    hh_ws_free(ctx, d_rec2);
+    hh_ws_free(ctx, d_fb_rec);
+    hh_dfree(d_fb_off);
+    hh_dfree(d_bcnt);
+    hh_dfree(d_bfill);
+    hh_dfree(d_boff);
+    hh_dfree(d_fallback);
+    hh_dfree(d_agg);
+    for (int t = 0; t < 2; ++t) {
+        hh_dfree(skeys[t]);
+        hh_dfree(svals[t]);
     }
     links_free_partsets(lk);
     HH_CHECK(rc);
     lk->finished = true;
     lk->ordered = false;        // dict insertion order is restored by the first hh_links_fetch (links_order_list)
+    return HH_OK;
+}
+
+extern "C" int hh_links_agg_info(hh_links* lk, int64_t* buckets, int64_t* smem_buckets, int64_t* fallback_buckets) {
+    HH_REQUIRE(lk != nullptr, HH_ERR_ARG, "hh_links_agg_info: NULL handle");
+    if (buckets) *buckets = lk->agg_buckets;
+    if (smem_buckets) *smem_buckets = lk->agg_smem;
+    if (fallback_buckets) *fallback_buckets = lk->agg_fallback;
     return HH_OK;
 }
 

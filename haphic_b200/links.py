@@ -112,6 +112,13 @@ class LinkTable:
         self.info = info
         return info
 
+    def agg_info(self) -> dict:
+        """How a partitioned count was aggregated at finish: hash buckets, those counted in shared memory, those counted
+        by the global-table fallback (all 0 for a table counted directly)."""
+        b, s, f = C.c_int64(), C.c_int64(), C.c_int64()
+        check(load().hh_links_agg_info(self._h, C.byref(b), C.byref(s), C.byref(f)))
+        return {"buckets": int(b.value), "smem_buckets": int(s.value), "fallback_buckets": int(f.value)}
+
     # -- results ---------------------------------------------------------------------------
     def fetch(self, pinned: bool = False) -> dict:
         """Arrays of nnz_full entries in full_link_dict insertion order.  ``pinned=True`` returns views of

@@ -108,6 +108,10 @@ typedef struct {
 
 /* close the stream: orders the distinct pairs by first appearance (dict insertion order) */
 int hh_links_finish(hh_links* lk, hh_links_info* info);
+/* how the finish of a partitioned count (long streams; hh_links_finish or hh_links_finish_partition) aggregated: the
+ * number of hash buckets, those counted in a shared-memory table, and those counted by the global-table fallback
+ * (too many records or distinct pairs for shared memory).  All 0 for a table counted directly.  Any pointer may be NULL. */
+int hh_links_agg_info(hh_links* lk, int64_t* buckets, int64_t* smem_buckets, int64_t* fallback_buckets);
 
 /* full_link_dict / flank_link_dict / HT_link_dict as parallel arrays of nnz_full entries in
  * full_link_dict insertion order (1649).  key_i/key_j: contig ids with name(key_i) < name(key_j).
