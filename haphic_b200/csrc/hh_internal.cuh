@@ -13,7 +13,11 @@ struct hh_matrix {
     int32_t n_index;
 };
 
-// How the matrix sees one entry of the compact link table (9 x uint32: i, j, full, flank, ...): the flank count, or
+// The words of one entry of the compact link table (HH_E_WORDS x uint32).  The order is the hh_links_export /
+// hh_links_adopt wire format.
+enum { HH_E_I, HH_E_J, HH_E_FULL, HH_E_FLANK, HH_E_FIRST_FULL, HH_E_FIRST_FLANK, HH_E_HT, HH_E_TH, HH_E_TT, HH_E_WORDS };
+
+// How the matrix sees one entry of the compact link table: the flank count, or
 // links / (tot_i * tot_j) ** 0.5 in fp64 with normalize (normalize_by_nlinks, 718-724), then -- when hap != NULL and the
 // two ends lie on different haplotypes -- x - x * w with two roundings (reduce_inter_hap_HiC_links, 695-707).  Returns
 // false when the entry is not in the (reduced) flank_link_dict: no flank link, or reduced to exactly 0.  hh_k_touch,
@@ -21,15 +25,15 @@ struct hh_matrix {
 // cannot disagree.
 __device__ __forceinline__ bool hh_flank_value(const uint32_t* __restrict__ p, const unsigned long long* __restrict__ ctg_tot,
                                                int normalize, const int32_t* __restrict__ hap, double w, double* x_out) {
-    if (p[3] == 0) return false;
+    if (p[HH_E_FLANK] == 0) return false;
     double x;
     if (normalize) {
-        const unsigned long long prod = ctg_tot[p[0]] * ctg_tot[p[1]];
-        x = (double)p[3] / pow((double)prod, 0.5);
+        const unsigned long long prod = ctg_tot[p[HH_E_I]] * ctg_tot[p[HH_E_J]];
+        x = (double)p[HH_E_FLANK] / pow((double)prod, 0.5);
     } else {
-        x = (double)p[3];
+        x = (double)p[HH_E_FLANK];
     }
-    if (hap != nullptr && hap[p[0]] != hap[p[1]]) x = __dsub_rn(x, __dmul_rn(x, w));
+    if (hap != nullptr && hap[p[HH_E_I]] != hap[p[HH_E_J]]) x = __dsub_rn(x, __dmul_rn(x, w));
     if (x == 0.0) return false;
     *x_out = x;
     return true;

@@ -27,20 +27,6 @@ struct __align__(32) hh_slot {
     uint32_t first_full, first_flank, full, flank, ht, th, tt, pad;
 };
 
-// Counter updates of one (warp-aggregated) group of records on a slot: plain 32-bit reductions (fire and forget).
-__device__ __forceinline__ void hh_slot_update(hh_slot* v, unsigned c_full, unsigned c_fl, uint32_t first_all, uint32_t first_fl,
-                                               unsigned c_ht, unsigned c_th, unsigned c_tt) {
-    atomicAdd(&v->full, c_full);
-    atomicMin(&v->first_full, first_all);
-    if (c_fl) {
-        atomicAdd(&v->flank, c_fl);
-        atomicMin(&v->first_flank, first_fl);
-    }
-    if (c_ht) atomicAdd(&v->ht, c_ht);
-    if (c_th) atomicAdd(&v->th, c_th);
-    if (c_tt) atomicAdd(&v->tt, c_tt);
-}
-
 struct hh_partset {
     int4* buf;                       // [npart][pcap] records {i, j, stream index, flags}
     unsigned long long* cursor;      // [npart] records written to every region (may exceed pcap: the excess went to the spill list)
@@ -72,7 +58,7 @@ struct hh_links {
     bool ordered;                    // d_compact is in dict insertion order (false after hh_links_finish_partition / hh_links_adopt)
     int64_t nnz, nnz_flank, n_used;
     int64_t peer_used;               // records counted by merged peers
-    uint32_t* d_compact;             // [nnz][9]  {i, j, full, flank, first_full, first_flank, HT, TH, TT}
+    uint32_t* d_compact;             // [nnz][HH_E_WORDS]  {i, j, full, flank, first_full, first_flank, HT, TH, TT}
     // host staging (double-buffered H2D)
     int4* d_stage[2];
     cudaEvent_t ev_copied[2], ev_consumed[2];
@@ -84,7 +70,7 @@ struct hh_links {
     uint64_t scap;                   // slots of a shared-memory table, or of the fallback's global table when one ran
     int64_t agg_buckets, agg_smem, agg_fallback;   // buckets at finish / counted in shared memory / by the fallback
     uint64_t spill_cap;
-    std::vector<hh_partset>* psets;  // partition buffers; normally one set, a new one when a later add call outgrows it
+    std::vector<hh_partset> psets;   // partition buffers; normally one set, a new one when a later add call outgrows it
     int4* d_spill;                   // records of partitions whose region overflowed (skewed keys), with their partition id
     unsigned long long* d_spill_cursor;
     int64_t capacity_hint;
@@ -137,6 +123,179 @@ __global__ void hh_k_links_init(uint64_t* __restrict__ keys, hh_slot* __restrict
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// What a record means: the ordered pair of key-space objects it links and three flags.  The partition records carry
+// the flags in the low bits of their .w.
+// ---------------------------------------------------------------------------------------------
+#define HH_F_FLANK 1u              // both ends in a flank region of an Nx member (flank_link_dict)
+#define HH_F_TI 2u                 // end i in the tail half of its object
+#define HH_F_TJ 4u                 // end j in the tail half of its object
+
+struct hh_pair {
+    int a, b;                        // key-space ids, in key order
+    unsigned flags;                  // HH_F_*
+};
+
+__device__ __forceinline__ uint64_t hh_pair_key(int a, int b) { return ((uint64_t)(uint32_t)a << 32) | (uint64_t)(uint32_t)b; }
+
+__device__ __forceinline__ void hh_swap_ends(int& a, int& b, int& pa, int& pb) {
+    int t = a; a = b; b = t;
+    t = pa; pa = pb; pb = t;
+}
+
+// the ordered pair (a, b) with its 0-based positions -> *out
+__device__ __forceinline__ void hh_pair_flags(int a, int b, int pa, int pb, const int32_t* __restrict__ ctg_len,
+                                              const uint8_t* __restrict__ in_nx, int64_t flank_bp, hh_pair* out) {
+    const int64_t coord_i = (int64_t)pa + 1, coord_j = (int64_t)pb + 1;   // 1-based
+    const int64_t li = ctg_len[a], lj = ctg_len[b];
+    const bool fi = (flank_bp == 0) || (coord_i <= flank_bp) || (coord_i > li - flank_bp);   // is_flank, 299-307
+    const bool fj = (flank_bp == 0) || (coord_j <= flank_bp) || (coord_j > lj - flank_bp);
+    out->a = a;
+    out->b = b;
+    out->flags = ((fi && fj && in_nx[a] && in_nx[b]) ? HH_F_FLANK : 0u)                         // 1636
+                 | ((coord_i * 2 > li) ? HH_F_TI : 0u) | ((coord_j * 2 > lj) ? HH_F_TJ : 0u);   // 404-416
+}
+
+// contig mode: false = the record is not counted (same contig: generator filter, 1582 / 2862; ids outside the FASTA, 1625)
+__device__ __forceinline__ bool hh_classify_contig(int4 r, int32_t n_ctg, const int32_t* __restrict__ ctg_len,
+                                                   const int32_t* __restrict__ name_rank, const uint8_t* __restrict__ in_nx,
+                                                   int64_t flank_bp, hh_pair* out) {
+    int a = r.x, b = r.z, pa = r.y, pb = r.w;
+    if (a == b || (unsigned)a >= (unsigned)n_ctg || (unsigned)b >= (unsigned)n_ctg) return false;
+    if (name_rank[a] > name_rank[b]) hh_swap_ends(a, b, pa, pb);      // sorted(((ref,pos+1),(mref,mpos+1))), 1629
+    hh_pair_flags(a, b, pa, pb, ctg_len, in_nx, flank_bp, out);
+    return true;
+}
+
+// convert_frags (1662-1670) for one end on a split contig: the contig's first fragment f and the position p become the bin
+// and the position inside it.  false = the position names a bin that does not exist
+__device__ __forceinline__ bool hh_to_bin(int& f, int& p, int nbins, int64_t bin_size) {
+    const int64_t nb = ((int64_t)p + 1 + bin_size - 1) / bin_size;
+    const bool exists = p >= 0 && nb >= 1 && nb <= (int64_t)nbins;
+    f += (int)(nb - 1);
+    p = (int)((int64_t)p - (nb - 1) * bin_size);
+    return exists;
+}
+
+// fragment mode (1696-1720): records name source contigs; a contig with several fragments is split into bins of bin_size
+// bp.  ctg_len / name_rank / in_nx describe the fragments; ids are checked against fbase.  idx = the record's stream index.
+__device__ __forceinline__ bool hh_classify_frag(int4 r, int32_t n_src, const int32_t* __restrict__ src_rank,
+                                                 const int32_t* __restrict__ fbase, int64_t bin_size, const int32_t* __restrict__ ctg_len,
+                                                 const int32_t* __restrict__ name_rank, const uint8_t* __restrict__ in_nx,
+                                                 int64_t flank_bp, uint32_t idx, unsigned long long* __restrict__ counters,
+                                                 hh_pair* out) {
+    int a = r.x, b = r.z, pa = r.y, pb = r.w;
+    if ((unsigned)a >= (unsigned)n_src || (unsigned)b >= (unsigned)n_src) return false;
+    if (a == b && fbase[a + 1] - fbase[a] <= 1) return false;        // intra-contig pairs only matter for split contigs (1699)
+    // sorted(((ref, pos+1), (mref, mpos+1))): by contig name, then by coordinate (1707)
+    if (src_rank[a] > src_rank[b] || (a == b && pa > pb)) hh_swap_ends(a, b, pa, pb);
+    int fa = fbase[a], fb = fbase[b];
+    const int na = fbase[a + 1] - fa, nb = fbase[b + 1] - fb;
+    // a position outside the contig (.pairs position 0, or beyond the last bin) names a bin that does not exist: the
+    // reference dies with a KeyError on frag_len_dict['ctg_binK']; here the record is refused and hh_links_finish reports it
+    bool bad = false;
+    if (na > 1) bad = !hh_to_bin(fa, pa, na, bin_size);
+    if (nb > 1) bad = !hh_to_bin(fb, pb, nb, bin_size) || bad;
+    if (bad) {
+        atomicAdd(counters + 5, 1ull);
+        atomicMax(counters + 6, (unsigned long long)idx + 1ull);
+        return false;
+    }
+    if (fa == fb) return false;                                       // intra-bin links are not considered (1715)
+    if ((na > 1 || nb > 1) && name_rank[fa] > name_rank[fb]) hh_swap_ends(fa, fb, pa, pb);   // sort by bin name (1719-1720)
+    hh_pair_flags(fa, fb, pa, pb, ctg_len, in_nx, flank_bp, out);
+    return true;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Folding a warp's records by key: the lanes that hold the same key form a group (match.any), and the group's lowest
+// lane -- its leader -- gets the group's counts and first-seen indices and updates the key's slot alone.  Coordinate- or
+// name-sorted inputs collapse 32 records into one update.
+// ---------------------------------------------------------------------------------------------
+struct hh_group {
+    bool leader;
+    uint32_t first_all, first_flank;     // smallest stream index of the group's records / of its flank records
+    unsigned full, flank, ht, th, tt;    // records of the group per counter
+};
+
+// Called by all 32 lanes; a lane without a record (ok = false) joins no group.
+__device__ __forceinline__ hh_group hh_warp_fold(bool ok, uint64_t key, uint32_t idx, unsigned flags) {
+    const int lane = threadIdx.x & 31;
+    if (!ok) key = HH_EMPTY_KEY - 1 - (uint64_t)lane;      // unique per lane: never groups, never a real key
+    const unsigned peers = __match_any_sync(HH_FULL_MASK, key);
+    const bool fl = ok && (flags & HH_F_FLANK), ti = (flags & HH_F_TI) != 0, tj = (flags & HH_F_TJ) != 0;
+    hh_group g;
+    g.first_all = __reduce_min_sync(peers, ok ? idx : HH_NONE32);
+    g.first_flank = __reduce_min_sync(peers, fl ? idx : HH_NONE32);
+    const unsigned b_fl = __ballot_sync(HH_FULL_MASK, fl);
+    const unsigned b_ht = __ballot_sync(HH_FULL_MASK, ok && !ti && tj);
+    const unsigned b_th = __ballot_sync(HH_FULL_MASK, ok && ti && !tj);
+    const unsigned b_tt = __ballot_sync(HH_FULL_MASK, ok && ti && tj);
+    g.leader = ok && lane == (__ffs(peers) - 1);
+    g.full = __popc(peers);
+    g.flank = __popc(peers & b_fl);
+    g.ht = __popc(peers & b_ht);
+    g.th = __popc(peers & b_th);
+    g.tt = __popc(peers & b_tt);
+    return g;
+}
+
+// A group's update of a slot of a global table: plain 32-bit reductions (fire and forget).
+__device__ __forceinline__ void hh_slot_update(hh_slot* v, const hh_group& g) {
+    atomicAdd(&v->full, g.full);
+    atomicMin(&v->first_full, g.first_all);
+    if (g.flank) {
+        atomicAdd(&v->flank, g.flank);
+        atomicMin(&v->first_flank, g.first_flank);
+    }
+    if (g.ht) atomicAdd(&v->ht, g.ht);
+    if (g.th) atomicAdd(&v->th, g.th);
+    if (g.tt) atomicAdd(&v->tt, g.tt);
+}
+
+__device__ __forceinline__ void hh_entry_store(uint32_t* __restrict__ o, uint64_t key, uint32_t full, uint32_t flank, uint32_t first_full,
+                                               uint32_t first_flank, uint32_t ht, uint32_t th, uint32_t tt) {
+    o[HH_E_I] = (uint32_t)(key >> 32);
+    o[HH_E_J] = (uint32_t)key;
+    o[HH_E_FULL] = full;
+    o[HH_E_FLANK] = flank;
+    o[HH_E_FIRST_FULL] = first_full;
+    o[HH_E_FIRST_FLANK] = first_flank;
+    o[HH_E_HT] = ht;
+    o[HH_E_TH] = th;
+    o[HH_E_TT] = tt;
+}
+
+// entry of a slot of a global table: v0 = {first_full, first_flank, full, flank}, v1 = {ht, th, tt, pad}
+__device__ __forceinline__ void hh_entry_store(uint32_t* __restrict__ o, uint64_t key, uint4 v0, uint4 v1) {
+    hh_entry_store(o, key, v0.z, v0.w, v0.x, v0.y, v1.x, v1.y, v1.z);
+}
+
+// Rank of this thread's `cnt` live items among those of its 256-thread block, in thread order, and the block's count.
+// s_wtot is shared scratch of 8 words; the first barrier makes a call safe right after the previous one was used.
+__device__ __forceinline__ unsigned int hh_block_rank(unsigned int cnt, unsigned int* s_wtot, unsigned int* total) {
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    unsigned int incl = cnt;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned int t = __shfl_up_sync(HH_FULL_MASK, incl, o);
+        if (lane >= o) incl += t;
+    }
+    __syncthreads();
+    if (lane == 31) s_wtot[wv] = incl;
+    __syncthreads();
+    unsigned int before = 0, all = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const unsigned int t = s_wtot[k];
+        before += (k < wv) ? t : 0u;
+        all += t;
+    }
+    *total = all;
+    return before + incl - cnt;
+}
+
+// load, classify, fold, probe, update
 __global__ void __launch_bounds__(256)
 hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_off, int32_t n_ctg,
                   const int32_t* __restrict__ ctg_len, const int32_t* __restrict__ name_rank,
@@ -158,107 +317,30 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x - lane); i0 < n_rec; i0 += stride) {
         const int64_t i = i0 + lane;
         bool ok = i < n_rec;
-        int4 r = make_int4(-1, 0, -1, 0);
-        if (ok) r = hh_ld_stream(rec + i);
-        uint64_t key = HH_EMPTY_KEY - 1 - (uint64_t)lane;   // unique per lane: never groups, never a real key
-        int ci = 0, cj = 0;
-        bool fl = false, ti = false, tj = false;
-        int a = r.x, b = r.z, pa = r.y, pb = r.w;
-        if (fbase == nullptr) {
-            ok = ok && (a != b) && ((unsigned)a < (unsigned)n_ctg) && ((unsigned)b < (unsigned)n_ctg);
-            if (ok && name_rank[a] > name_rank[b]) {      // sorted(((ref,pos+1),(mref,mpos+1))), 1629
-                int t = a; a = b; b = t;
-                t = pa; pa = pb; pb = t;
-            }
-        } else {
-            // fragment mode (1696-1720): records name source contigs; a contig with several fragments is split
-            // into bins of bin_size bp.  n_ctg is the number of fragments here; ids are checked against fbase.
-            ok = ok && ((unsigned)a < (unsigned)n_src) && ((unsigned)b < (unsigned)n_src);
-            if (ok) {
-                const bool split_a = fbase[a + 1] - fbase[a] > 1;
-                ok = (a != b) || split_a;                  // intra-contig pairs only matter for split contigs (1699)
-            }
-            if (ok) {
-                // sorted(((ref, pos+1), (mref, mpos+1))): by contig name, then by coordinate (1707)
-                const int ra = src_rank[a], rb = src_rank[b];
-                if (ra > rb || (a == b && pa > pb)) {
-                    int t = a; a = b; b = t;
-                    t = pa; pa = pb; pb = t;
-                }
-                // convert_frags (1662-1670)
-                int fa = fbase[a], fb = fbase[b];
-                const bool sa = fbase[a + 1] - fa > 1, sb = fbase[b + 1] - fb > 1;
-                // a position outside the contig (.pairs position 0, or beyond the last bin) names a bin that does not
-                // exist: the reference dies with a KeyError on frag_len_dict['ctg_binK']; here the record is refused and
-                // hh_links_finish reports it
-                bool bad = false;
-                if (sa) {
-                    const int64_t nb = ((int64_t)pa + 1 + bin_size - 1) / bin_size;
-                    bad = bad || pa < 0 || nb < 1 || nb > (int64_t)(fbase[a + 1] - fa);
-                    fa += (int)(nb - 1);
-                    pa = (int)((int64_t)pa - (nb - 1) * bin_size);
-                }
-                if (sb) {
-                    const int64_t nb = ((int64_t)pb + 1 + bin_size - 1) / bin_size;
-                    bad = bad || pb < 0 || nb < 1 || nb > (int64_t)(fbase[b + 1] - fb);
-                    fb += (int)(nb - 1);
-                    pb = (int)((int64_t)pb - (nb - 1) * bin_size);
-                }
-                if (bad) {
-                    atomicAdd(counters + 5, 1ull);
-                    atomicMax(counters + 6, (unsigned long long)(pos ? pos[i] : stream_off + (uint32_t)i) + 1ull);
-                }
-                ok = !bad && fa != fb;                     // intra-bin links are not considered (1715)
-                a = fa;
-                b = fb;
-                if (ok && (sa || sb) && name_rank[a] > name_rank[b]) {   // sort by bin name (1719-1720)
-                    int t = a; a = b; b = t;
-                    t = pa; pa = pb; pb = t;
-                }
-            }
-        }
+        hh_pair p = {0, 0, 0u};
+        uint32_t idx = HH_NONE32;
         if (ok) {
-            ci = a;
-            cj = b;
-            const int64_t coord_i = (int64_t)pa + 1, coord_j = (int64_t)pb + 1;   // 1-based
-            const int64_t li = ctg_len[a], lj = ctg_len[b];
-            const bool fi = (flank_bp == 0) || (coord_i <= flank_bp) || (coord_i > li - flank_bp);   // is_flank, 299-307
-            const bool fj = (flank_bp == 0) || (coord_j <= flank_bp) || (coord_j > lj - flank_bp);
-            fl = fi && fj && in_nx[a] && in_nx[b];                                                  // 1636
-            ti = coord_i * 2 > li;                                                                   // 404-416
-            tj = coord_j * 2 > lj;
-            key = ((uint64_t)(uint32_t)a << 32) | (uint64_t)(uint32_t)b;
-            my_used++;
+            const int4 r = hh_ld_stream(rec + i);
+            // stream position of the record: implicit (contiguous shard) or carried along (routed records, any order)
+            idx = pos ? pos[i] : stream_off + (uint32_t)i;
+            ok = fbase == nullptr ? hh_classify_contig(r, n_ctg, ctg_len, name_rank, in_nx, flank_bp, &p)
+                                  : hh_classify_frag(r, n_src, src_rank, fbase, bin_size, ctg_len, name_rank, in_nx, flank_bp, idx,
+                                                     counters, &p);
         }
-        const unsigned peers = __match_any_sync(HH_FULL_MASK, key);
-        // stream position of the record: implicit (contiguous shard) or carried along (routed records, any order)
-        uint32_t first_all = stream_off + (uint32_t)i, first_fl = HH_NONE32;
-        if (pos != nullptr) {
-            const uint32_t mine = ok ? pos[i] : HH_NONE32;
-            first_all = __reduce_min_sync(peers, mine);
-            first_fl = __reduce_min_sync(peers, (ok && fl) ? mine : HH_NONE32);
-        }
-        const unsigned b_fl = __ballot_sync(HH_FULL_MASK, ok && fl);
-        const unsigned b_ht = __ballot_sync(HH_FULL_MASK, ok && !ti && tj);
-        const unsigned b_th = __ballot_sync(HH_FULL_MASK, ok && ti && !tj);
-        const unsigned b_tt = __ballot_sync(HH_FULL_MASK, ok && ti && tj);
-        if (ok && lane == (__ffs(peers) - 1)) {
+        if (ok) my_used++;
+        const uint64_t key = hh_pair_key(p.a, p.b);
+        const hh_group g = hh_warp_fold(ok, key, idx, p.flags);
+        if (g.leader) {
             bool inserted;
             const uint64_t slot = hh_probe_insert(keys, cap, key, &inserted);
             if (slot >= cap) {
                 s_over = 1;
             } else {
                 if (inserted) my_new++;
-                hh_slot* v = vals + slot;
-                const unsigned c_full = __popc(peers);
-                const unsigned m_fl = peers & b_fl;
-                const unsigned c_fl = __popc(m_fl);
-                const unsigned c_ht = __popc(peers & b_ht), c_th = __popc(peers & b_th), c_tt = __popc(peers & b_tt);
-                // leader = lowest lane = earliest record
-                hh_slot_update(v, c_full, c_fl, first_all, pos ? first_fl : stream_off + (uint32_t)(i0 + (__ffs(m_fl) - 1)), c_ht, c_th, c_tt);
-                if (c_fl) {
-                    atomicAdd(ctg_links + ci, (unsigned long long)c_fl);
-                    atomicAdd(ctg_links + cj, (unsigned long long)c_fl);
+                hh_slot_update(vals + slot, g);
+                if (g.flank) {
+                    atomicAdd(ctg_links + p.a, (unsigned long long)g.flank);
+                    atomicAdd(ctg_links + p.b, (unsigned long long)g.flank);
                 }
             }
         }
@@ -314,24 +396,12 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
             const int64_t i = t * HH_PART_TILE + (int64_t)k * 512 + threadIdx.x;
             part[k] = -1;
             if (i < n_rec) {
-                const int4 r = hh_ld_stream(rec + i);
-                int a = r.x, b = r.z, pa = r.y, pb = r.w;
-                if (a != b && (unsigned)a < (unsigned)n_ctg && (unsigned)b < (unsigned)n_ctg) {
-                    if (name_rank[a] > name_rank[b]) {      // sorted(((ref,pos+1),(mref,mpos+1))), 1629
-                        int x = a; a = b; b = x;
-                        x = pa; pa = pb; pb = x;
-                    }
-                    const int64_t coord_i = (int64_t)pa + 1, coord_j = (int64_t)pb + 1;
-                    const int64_t li = ctg_len[a], lj = ctg_len[b];
-                    const bool fi = (flank_bp == 0) || (coord_i <= flank_bp) || (coord_i > li - flank_bp);   // is_flank, 299-307
-                    const bool fj = (flank_bp == 0) || (coord_j <= flank_bp) || (coord_j > lj - flank_bp);
-                    const unsigned fl = (fi && fj && in_nx[a] && in_nx[b]) ? 1u : 0u;                         // 1636
-                    const unsigned ti = (coord_i * 2 > li) ? 2u : 0u, tj = (coord_j * 2 > lj) ? 4u : 0u;       // 404-416
-                    const uint64_t key = ((uint64_t)(uint32_t)a << 32) | (uint64_t)(uint32_t)b;
-                    const int p = (int)(hh_mix64(key) >> (64 - npart_log));
+                hh_pair pr;
+                if (hh_classify_contig(hh_ld_stream(rec + i), n_ctg, ctg_len, name_rank, in_nx, flank_bp, &pr)) {
+                    const int p = (int)(hh_mix64(hh_pair_key(pr.a, pr.b)) >> (64 - npart_log));
                     part[k] = p;
                     rnk[k] = atomicAdd(&s_cnt[p], 1u);
-                    out[k] = make_int4(a, b, (int)(stream_off + (uint32_t)i), (int)(fl | ti | tj | ((unsigned)p << 8)));
+                    out[k] = make_int4(pr.a, pr.b, (int)(stream_off + (uint32_t)i), (int)(pr.flags | ((unsigned)p << 8)));
                     my_used++;
                 }
             }
@@ -370,8 +440,7 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 #define HH_AGG_HOT 32              // a bucket with more than HH_AGG_HOT x the mean records skips shared memory (links_hot_records)
 
 __device__ __forceinline__ uint32_t hh_bucket_of(int4 r, int bucket_log) {
-    const uint64_t key = ((uint64_t)(uint32_t)r.x << 32) | (uint64_t)(uint32_t)r.y;
-    return (uint32_t)(hh_mix64(key) >> (64 - bucket_log));
+    return (uint32_t)(hh_mix64(hh_pair_key(r.x, r.y)) >> (64 - bucket_log));
 }
 
 // Records per bucket.  The virtual tiles are `tpr` tiles of every region (those past the region's fill exit at once),
@@ -532,18 +601,9 @@ hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff
             const bool ok = i < n;
             int4 r = make_int4(0, 0, 0, 0);
             if (ok) r = hh_ld_stream(rec + lo + i);
-            const unsigned f = (unsigned)r.w;
-            const uint64_t key = ok ? (((uint64_t)(uint32_t)r.x << 32) | (uint64_t)(uint32_t)r.y) : (HH_EMPTY_KEY - 1 - (uint64_t)lane);
-            const unsigned peers = __match_any_sync(HH_FULL_MASK, key);
-            const bool fl = ok && (f & 1u), ti = (f & 2u) != 0, tj = (f & 4u) != 0;
-            const uint32_t idx = ok ? (uint32_t)r.z : HH_NONE32;
-            const uint32_t first_all = __reduce_min_sync(peers, idx);
-            const uint32_t first_fl = __reduce_min_sync(peers, fl ? idx : HH_NONE32);
-            const unsigned b_fl = __ballot_sync(HH_FULL_MASK, fl);
-            const unsigned b_ht = __ballot_sync(HH_FULL_MASK, ok && !ti && tj);
-            const unsigned b_th = __ballot_sync(HH_FULL_MASK, ok && ti && !tj);
-            const unsigned b_tt = __ballot_sync(HH_FULL_MASK, ok && ti && tj);
-            if (ok && lane == (__ffs(peers) - 1)) {
+            const uint64_t key = hh_pair_key(r.x, r.y);
+            const hh_group g = hh_warp_fold(ok, key, (uint32_t)r.z, (unsigned)r.w);
+            if (g.leader) {
                 unsigned int slot = (unsigned int)hh_mix64(key) & mask;
                 int probes = 0;
                 for (; probes < tsize; ++probes) {
@@ -563,17 +623,15 @@ hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff
                 if (probes == tsize) {
                     s_abandon = 1;
                 } else {
-                    atomicAdd(t_full + slot, (unsigned)__popc(peers));
-                    atomicMin(t_ffull + slot, first_all);
-                    const unsigned c_fl = __popc(peers & b_fl);
-                    if (c_fl) {
-                        atomicAdd(t_flank + slot, c_fl);
-                        atomicMin(t_fflank + slot, first_fl);
+                    atomicAdd(t_full + slot, g.full);
+                    atomicMin(t_ffull + slot, g.first_all);
+                    if (g.flank) {
+                        atomicAdd(t_flank + slot, g.flank);
+                        atomicMin(t_fflank + slot, g.first_flank);
                     }
-                    const unsigned c_ht = __popc(peers & b_ht), c_th = __popc(peers & b_th), c_tt = __popc(peers & b_tt);
-                    if (c_ht) atomicAdd(t_ht + slot, c_ht);
-                    if (c_th) atomicAdd(t_th + slot, c_th);
-                    if (c_tt) atomicAdd(t_tt + slot, c_tt);
+                    if (g.ht) atomicAdd(t_ht + slot, g.ht);
+                    if (g.th) atomicAdd(t_th + slot, g.th);
+                    if (g.tt) atomicAdd(t_tt + slot, g.tt);
                 }
             }
             if (__any_sync(HH_FULL_MASK, *((volatile unsigned int*)&s_abandon) != 0)) break;
@@ -592,33 +650,14 @@ hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff
             const int s = s0 + threadIdx.x;
             const uint64_t key = tkey[s];
             const bool live = key != HH_EMPTY_KEY;
-            const unsigned bal = __ballot_sync(HH_FULL_MASK, live);
-            if (lane == 0) s_wtot[wv] = __popc(bal);
-            __syncthreads();
-            unsigned int before = 0, total = 0;
-#pragma unroll
-            for (int k = 0; k < HH_AGG_THREADS / 32; ++k) {
-                const unsigned int t = s_wtot[k];
-                before += (k < wv) ? t : 0u;
-                total += t;
-            }
+            unsigned int total;
+            const unsigned long long pos = run + hh_block_rank(live ? 1u : 0u, s_wtot, &total);
             if (live) {
-                const unsigned long long pos = run + before + __popc(bal & ((1u << lane) - 1u));
                 const uint32_t flank = t_flank[s];
-                if (pos < compact_cap) {
-                    uint32_t* o = compact + pos * 9;
-                    o[0] = (uint32_t)(key >> 32);
-                    o[1] = (uint32_t)key;
-                    o[2] = t_full[s];
-                    o[3] = flank;
-                    o[4] = t_ffull[s];
-                    o[5] = t_fflank[s];
-                    o[6] = t_ht[s];
-                    o[7] = t_th[s];
-                    o[8] = t_tt[s];
-                } else {
+                if (pos < compact_cap)
+                    hh_entry_store(compact + pos * HH_E_WORDS, key, t_full[s], flank, t_ffull[s], t_fflank[s], t_ht[s], t_th[s], t_tt[s]);
+                else
                     atomicExch(counters + 2, 5ull);
-                }
                 if (flank) {
                     nfl++;
                     atomicAdd(ctg_links + (uint32_t)(key >> 32), (unsigned long long)flank);      // ctg_link_dict (1638-1639)
@@ -627,7 +666,6 @@ hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff
                 clear(s);
             }
             run += total;
-            __syncthreads();                        // s_wtot is rewritten by the next trip
         }
         n_done++;
     }
@@ -668,27 +706,13 @@ __device__ __forceinline__ void hh_part_count(const int4* __restrict__ prec, int
         const bool ok = i < n;
         int4 r = make_int4(0, 0, 0, 0);
         if (ok) r = hh_ld_stream(prec + i);
-        const unsigned f = (unsigned)r.w;
-        const uint64_t key = ok ? (((uint64_t)(uint32_t)r.x << 32) | (uint64_t)(uint32_t)r.y) : (HH_EMPTY_KEY - 1 - (uint64_t)lane);
-        const unsigned peers = __match_any_sync(HH_FULL_MASK, key);
-        const bool fl = ok && (f & 1u), ti = (f & 2u) != 0, tj = (f & 4u) != 0;
-        const uint32_t idx = ok ? (uint32_t)r.z : HH_NONE32;
-        const uint32_t first_all = __reduce_min_sync(peers, idx);
-        const uint32_t first_fl = __reduce_min_sync(peers, fl ? idx : HH_NONE32);
-        const unsigned b_fl = __ballot_sync(HH_FULL_MASK, fl);
-        const unsigned b_ht = __ballot_sync(HH_FULL_MASK, ok && !ti && tj);
-        const unsigned b_th = __ballot_sync(HH_FULL_MASK, ok && ti && !tj);
-        const unsigned b_tt = __ballot_sync(HH_FULL_MASK, ok && ti && tj);
-        if (ok && lane == (__ffs(peers) - 1)) {
+        const uint64_t key = hh_pair_key(r.x, r.y);
+        const hh_group g = hh_warp_fold(ok, key, (uint32_t)r.z, (unsigned)r.w);
+        if (g.leader) {
             bool inserted;
             const uint64_t slot = hh_probe_insert(keys, cap, key, &inserted);
-            if (slot >= cap) {
-                atomicExch(counters + 2, 4ull);
-            } else {
-                hh_slot* v = vals + slot;
-                hh_slot_update(v, (unsigned)__popc(peers), (unsigned)__popc(peers & b_fl), first_all, first_fl, (unsigned)__popc(peers & b_ht),
-                               (unsigned)__popc(peers & b_th), (unsigned)__popc(peers & b_tt));
-            }
+            if (slot >= cap) atomicExch(counters + 2, 4ull);
+            else hh_slot_update(vals + slot, g);
         }
     }
 }
@@ -705,7 +729,6 @@ hh_k_part_step(const int4* __restrict__ prec, int64_t n, uint64_t* __restrict__ 
     if (ekeys != nullptr) {
         __shared__ unsigned int s_wtot[8];
         __shared__ unsigned long long s_base;
-        const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
         unsigned int nfl = 0;
         constexpr int E = 2;
         for (uint64_t r0 = (uint64_t)blockIdx.x * (256ull * E); r0 < cap; r0 += (uint64_t)gridDim.x * (256ull * E)) {
@@ -717,26 +740,12 @@ hh_k_part_step(const int4* __restrict__ prec, int64_t n, uint64_t* __restrict__ 
                 key[q] = (sl < cap) ? ekeys[sl] : HH_EMPTY_KEY;
                 cnt += (key[q] != HH_EMPTY_KEY) ? 1u : 0u;
             }
-            unsigned int incl = cnt;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned int t = __shfl_up_sync(HH_FULL_MASK, incl, o);
-                if (lane >= o) incl += t;
-            }
-            __syncthreads();                       // s_wtot / s_base of the previous trip have been read
-            if (lane == 31) s_wtot[wv] = incl;
-            __syncthreads();
-            unsigned int before = 0, total = 0;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const unsigned int t = s_wtot[k];
-                before += (k < wv) ? t : 0u;
-                total += t;
-            }
+            unsigned int total;
+            const unsigned int rank = hh_block_rank(cnt, s_wtot, &total);     // its first barrier: the last trip has read s_base
             if (threadIdx.x == 0) s_base = total ? atomicAdd(counters + 0, (unsigned long long)total) : 0ull;
             __syncthreads();
             if (cnt) {
-                unsigned long long pos = s_base + before + (incl - cnt);
+                unsigned long long pos = s_base + rank;
                 uint4 v0[E], v1[E];
 #pragma unroll
                 for (int q = 0; q < E; ++q) {
@@ -750,20 +759,8 @@ hh_k_part_step(const int4* __restrict__ prec, int64_t n, uint64_t* __restrict__ 
                 for (int q = 0; q < E; ++q) {
                     if (key[q] == HH_EMPTY_KEY) continue;
                     const uint64_t sl = r0 + (uint64_t)q * 256ull + threadIdx.x;
-                    if (pos < compact_cap) {
-                        uint32_t* o = compact + pos * 9;
-                        o[0] = (uint32_t)(key[q] >> 32);
-                        o[1] = (uint32_t)key[q];
-                        o[2] = v0[q].z;
-                        o[3] = v0[q].w;
-                        o[4] = v0[q].x;
-                        o[5] = v0[q].y;
-                        o[6] = v1[q].x;
-                        o[7] = v1[q].y;
-                        o[8] = v1[q].z;
-                    } else {
-                        atomicExch(counters + 2, 5ull);
-                    }
+                    if (pos < compact_cap) hh_entry_store(compact + pos * HH_E_WORDS, key[q], v0[q], v1[q]);
+                    else atomicExch(counters + 2, 5ull);
                     pos++;
                     if (v0[q].w) {
                         nfl++;
@@ -778,7 +775,7 @@ hh_k_part_step(const int4* __restrict__ prec, int64_t n, uint64_t* __restrict__ 
             }
         }
         nfl = (unsigned)hh_warp_sum((int)nfl);
-        if (lane == 0 && nfl) atomicAdd(counters + 3, (unsigned long long)nfl);
+        if ((threadIdx.x & 31) == 0 && nfl) atomicAdd(counters + 3, (unsigned long long)nfl);
     }
     // ---- count the current bucket
     if (ckeys != nullptr && n > 0) hh_part_count(prec, n, ckeys, cvals, cap, counters);
@@ -814,8 +811,8 @@ __global__ void hh_k_links_merge(const uint32_t* __restrict__ ent, int64_t n_ent
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     unsigned int my_new = 0, my_last = 0;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_ent; e += stride) {
-        const uint32_t* p = ent + e * 9;
-        const uint64_t key = ((uint64_t)p[0] << 32) | (uint64_t)p[1];
+        const uint32_t* p = ent + e * HH_E_WORDS;
+        const uint64_t key = ((uint64_t)p[HH_E_I] << 32) | (uint64_t)p[HH_E_J];
         bool inserted;
         const uint64_t slot = hh_probe_insert(keys, cap, key, &inserted);
         if (slot >= cap) {
@@ -824,14 +821,14 @@ __global__ void hh_k_links_merge(const uint32_t* __restrict__ ent, int64_t n_ent
         }
         if (inserted) my_new++;
         hh_slot* v = vals + slot;
-        atomicAdd(&v->full, p[2]);
-        if (p[3]) atomicAdd(&v->flank, p[3]);
-        atomicMin(&v->first_full, p[4]);
-        atomicMin(&v->first_flank, p[5]);
-        my_last = max(my_last, p[4]);
-        if (p[6]) atomicAdd(&v->ht, p[6]);
-        if (p[7]) atomicAdd(&v->th, p[7]);
-        if (p[8]) atomicAdd(&v->tt, p[8]);
+        atomicAdd(&v->full, p[HH_E_FULL]);
+        if (p[HH_E_FLANK]) atomicAdd(&v->flank, p[HH_E_FLANK]);
+        atomicMin(&v->first_full, p[HH_E_FIRST_FULL]);
+        atomicMin(&v->first_flank, p[HH_E_FIRST_FLANK]);
+        my_last = max(my_last, p[HH_E_FIRST_FULL]);
+        if (p[HH_E_HT]) atomicAdd(&v->ht, p[HH_E_HT]);
+        if (p[HH_E_TH]) atomicAdd(&v->th, p[HH_E_TH]);
+        if (p[HH_E_TT]) atomicAdd(&v->tt, p[HH_E_TT]);
     }
     if (my_new) atomicAdd(&s_new, my_new);
     my_last = __reduce_max_sync(HH_FULL_MASK, my_last);
@@ -923,7 +920,7 @@ __global__ void hh_k_list_scatter_order(const uint32_t* __restrict__ ent, int64_
                                         unsigned long long* __restrict__ counters) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t f = ent[e * 9 + 4];
+        const uint32_t f = ent[e * HH_E_WORDS + HH_E_FIRST_FULL];
         if ((int64_t)f < stream_end) order[f] = (uint32_t)e;
         else atomicExch(counters + 2, 2ull);
     }
@@ -932,7 +929,8 @@ __global__ void hh_k_list_scatter_order(const uint32_t* __restrict__ ent, int64_
 __global__ void hh_k_list_count_flank(const uint32_t* __restrict__ ent, int64_t nnz, unsigned long long* __restrict__ counters) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     unsigned int c = 0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) c += ent[e * 9 + 3] ? 1u : 0u;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride)
+        c += ent[e * HH_E_WORDS + HH_E_FLANK] ? 1u : 0u;
     c = hh_warp_sum((int)c);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(counters + 3, (unsigned long long)c);
 }
@@ -974,58 +972,37 @@ __global__ void __launch_bounds__(256)
 hh_k_compact_gather(const uint32_t* __restrict__ order, int64_t n, const int64_t* __restrict__ block_off,
                     const uint64_t* __restrict__ keys, const hh_slot* __restrict__ vals,
                     uint32_t* __restrict__ compact, unsigned long long* __restrict__ counters) {
-    __shared__ int s_warp[8];
+    __shared__ unsigned int s_wtot[8];
     __shared__ unsigned int s_flank;
     if (threadIdx.x == 0) s_flank = 0;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t base = (int64_t)blockIdx.x * HH_CMP_TILE + (int64_t)threadIdx.x * 8;
     uint32_t slot[8];
-    int c = 0;
+    unsigned int c = 0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const int64_t e = base + k;
         slot[k] = (e < n) ? order[e] : HH_NONE32;
         if (slot[k] != HH_NONE32) c++;
     }
-    int incl = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        int t = __shfl_up_sync(HH_FULL_MASK, incl, o);
-        if (lane >= o) incl += t;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    int woff = 0;
-    for (int w = 0; w < warp; ++w) woff += s_warp[w];
-    int64_t q = block_off[blockIdx.x] + woff + incl - c;
+    unsigned int total;
+    int64_t q = block_off[blockIdx.x] + hh_block_rank(c, s_wtot, &total);
     unsigned int nfl = 0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         if (slot[k] == HH_NONE32) continue;
+        uint32_t* o = compact + q * HH_E_WORDS;
+        q++;
         if (keys == nullptr) {
-            // source is an entry list (hh_links_adopt): plain copy of the 9 words
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(vals) + (size_t)slot[k] * 9;
-            uint32_t* o = compact + q * 9;
+            // source is an entry list (hh_links_adopt): plain copy of the words
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(vals) + (size_t)slot[k] * HH_E_WORDS;
 #pragma unroll
-            for (int w = 0; w < 9; ++w) o[w] = src[w];
-            q++;
+            for (int w = 0; w < HH_E_WORDS; ++w) o[w] = src[w];
             continue;
         }
-        const uint64_t key = keys[slot[k]];
         const uint4* v = reinterpret_cast<const uint4*>(vals + slot[k]);
-        const uint4 v0 = v[0], v1 = v[1];   // {first_full, first_flank, full, flank} {ht, th, tt, pad}
-        uint32_t* o = compact + q * 9;
-        o[0] = (uint32_t)(key >> 32);
-        o[1] = (uint32_t)key;
-        o[2] = v0.z;
-        o[3] = v0.w;
-        o[4] = v0.x;
-        o[5] = v0.y;
-        o[6] = v1.x;
-        o[7] = v1.y;
-        o[8] = v1.z;
+        const uint4 v0 = v[0], v1 = v[1];
+        hh_entry_store(o, keys[slot[k]], v0, v1);
         if (v0.w) nfl++;
-        q++;
     }
     if (nfl) atomicAdd(&s_flank, nfl);
     __syncthreads();
@@ -1041,13 +1018,13 @@ __global__ void hh_k_touch(const uint32_t* __restrict__ compact, int64_t nnz, co
                            double w, unsigned long long* __restrict__ touch) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t* p = compact + e * 9;
-        if (p[3] == 0) continue;                       // no flank link
-        const uint32_t i = p[0], j = p[1];
+        const uint32_t* p = compact + e * HH_E_WORDS;
+        if (p[HH_E_FLANK] == 0) continue;              // no flank link
+        const uint32_t i = p[HH_E_I], j = p[HH_E_J];
         if (!keep[i] || !keep[j]) continue;            // 329-330
         double x;
         if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;   // not in flank_link_dict
-        const unsigned long long t = (unsigned long long)p[5] * 2ull;
+        const unsigned long long t = (unsigned long long)p[HH_E_FIRST_FLANK] * 2ull;
         atomicMin(touch + i, t);
         atomicMin(touch + j, t + 1ull);
     }
@@ -1079,6 +1056,11 @@ hh_k_rank_touch(const unsigned long long* __restrict__ touch, int n, int32_t* __
 // host side
 // ---------------------------------------------------------------------------------------------
 static inline int hh_grid(hh_ctx* ctx, int per_sm) { return ctx->sm_count * per_sm; }
+
+// blocks of 256 threads for a grid-stride kernel over n items: one thread per item, at most 8 blocks per SM
+static inline int links_grid(hh_ctx* ctx, int64_t n) {
+    return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, hh_grid(ctx, 8)));
+}
 
 static int links_alloc_table(hh_links* lk, uint64_t cap, uint64_t** keys, hh_slot** vals) {
     HH_CHECK(hh_dmalloc(keys, cap));
@@ -1149,9 +1131,8 @@ static int links_create_common(hh_ctx* ctx, int32_t n_key, const int64_t* key_le
         HH_REQUIRE(key_rank[c] >= 0 && key_rank[c] < n_key, HH_ERR_ARG, "hh_links_create: name_rank[%d] out of range", c);
         len32[c] = (int32_t)key_len[c];
     }
-    hh_links* lk = new (std::nothrow) hh_links();
+    hh_links* lk = new (std::nothrow) hh_links();      // value-initialised: every field zero, no partition set
     HH_REQUIRE(lk != nullptr, HH_ERR_NOMEM, "hh_links_create: out of host memory");
-    memset(lk, 0, sizeof(*lk));
     lk->ctx = ctx;
     lk->n_ctg = n_key;
     lk->n_src = frag_base ? n_src : n_key;
@@ -1187,7 +1168,6 @@ static int links_create_common(hh_ctx* ctx, int32_t n_key, const int64_t* key_le
     }
     HH_CUDA(cudaStreamSynchronize(st));   // host temporaries go out of scope
     lk->capacity_hint = capacity_hint;
-    lk->psets = new std::vector<hh_partset>();
     HH_CUDA(cudaStreamCreateWithFlags(&lk->copy_stream, cudaStreamNonBlocking));
     for (int k = 0; k < 2; ++k) {
         HH_CUDA(cudaEventCreateWithFlags(&lk->ev_copied[k], cudaEventDisableTiming));
@@ -1242,7 +1222,7 @@ static int links_new_partset(hh_links* lk, int64_t n_rec) {
         return rc;
     }
     HH_CUDA(cudaMemsetAsync(ps.cursor, 0, (size_t)npart * sizeof(unsigned long long), lk->ctx->stream));
-    lk->psets->push_back(ps);
+    lk->psets.push_back(ps);
     return HH_OK;
 }
 
@@ -1252,7 +1232,7 @@ static int links_new_partset(hh_links* lk, int64_t n_rec) {
 // and ahead of the next one; the spill cursor is unchanged.
 static int links_size_spill(hh_links* lk) {
     int64_t sized = 0;
-    for (size_t k = 0; k < lk->psets->size(); ++k) sized += (*lk->psets)[k].sized_for;
+    for (const hh_partset& ps : lk->psets) sized += ps.sized_for;
     const uint64_t need = (uint64_t)(sized / 8) + (4u << 20);
     if (lk->d_spill && need <= lk->spill_cap) return HH_OK;
     int4* grown = nullptr;
@@ -1301,31 +1281,41 @@ static int links_launch_insert(hh_links* lk, const int4* d_rec, int64_t n_rec, i
         const int64_t tiles = (n_rec + HH_PART_TILE - 1) / HH_PART_TILE;
         int grid = (int)(tiles < (int64_t)hh_grid(ctx, 3) ? tiles : (int64_t)hh_grid(ctx, 3));
         if (grid < 1) grid = 1;
-        const hh_partset& ps = lk->psets->back();
+        const hh_partset& ps = lk->psets.back();
         HH_LAUNCH(ctx, hh_k_part_scatter, grid, 512, 0, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank, lk->d_nx,
                   lk->flank_bp, lk->npart_log, ps.buf, ps.pcap, ps.cursor, lk->d_spill, lk->spill_cap, lk->d_spill_cursor,
                   lk->d_counters);
         return HH_OK;
     }
     HH_CHECK(links_need_table(lk));
-    int64_t blocks = (n_rec + 255) / 256;
-    int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
-    if (grid < 1) grid = 1;
-    HH_LAUNCH(ctx, hh_k_links_insert, grid, 256, 0, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank,
-              lk->d_nx, lk->flank_bp, lk->d_keys, lk->d_vals, lk->cap, lk->d_ctg, lk->d_counters, lk->d_src_rank, lk->d_fbase,
-              lk->bin_size, lk->n_src, d_pos);
+    HH_LAUNCH(ctx, hh_k_links_insert, links_grid(ctx, n_rec), 256, 0, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len,
+              lk->d_rank, lk->d_nx, lk->flank_bp, lk->d_keys, lk->d_vals, lk->cap, lk->d_ctg, lk->d_counters, lk->d_src_rank,
+              lk->d_fbase, lk->bin_size, lk->n_src, d_pos);
     return HH_OK;
 }
 
 // partitioned mode: a call that would outgrow the current set (sized for the first call) gets a set of its own
 static int links_part_room(hh_links* lk, int64_t n_rec) {
-    hh_partset& ps = lk->psets->back();
+    hh_partset& ps = lk->psets.back();
     if (ps.sent > 0 && ps.sent + n_rec > ps.sized_for + ps.sized_for / 8) {
         HH_CHECK(links_new_partset(lk, n_rec));
-        lk->psets->back().sent = n_rec;
+        lk->psets.back().sent = n_rec;
         return links_size_spill(lk);
     }
     ps.sent += n_rec;
+    return HH_OK;
+}
+
+// Device records in chunks of 8 Mi (128 MiB), so that the direct table can grow between two kernels.  d_pos = the stream
+// index of every record (routed records), or NULL when they are stream_offset, stream_offset + 1, ...
+static const int64_t HH_ADD_CHUNK = 1ll << 23;
+static int links_add_chunks(hh_links* lk, const int4* d_rec, const uint32_t* d_pos, int64_t n_rec, int64_t stream_offset) {
+    for (int64_t off = 0; off < n_rec; off += HH_ADD_CHUNK) {
+        const int64_t m = std::min(n_rec - off, HH_ADD_CHUNK);
+        if (lk->mode != 2) HH_CHECK(links_ensure_capacity(lk, m));
+        HH_CHECK(links_launch_insert(lk, d_rec + off, m, stream_offset + off, d_pos ? d_pos + off : nullptr));
+        lk->since_known += m;
+    }
     return HH_OK;
 }
 
@@ -1359,17 +1349,12 @@ extern "C" int hh_links_add(hh_links* lk, const int32_t* rec, int64_t n_rec, int
     if (n_rec == 0) return HH_OK;
     hh_ctx* ctx = lk->ctx;
     HH_CUDA(cudaSetDevice(ctx->device));
-    const int64_t CH = 1ll << 23;   // 8 Mi records = 128 MiB per chunk
+    const int64_t CH = HH_ADD_CHUNK;
     HH_CHECK(links_choose_mode(lk, n_rec));
     if (lk->mode == 2) HH_CHECK(links_part_room(lk, n_rec));
     if (mem == HH_MEM_DEVICE) {
         HH_REQUIRE(((uintptr_t)rec & 15) == 0, HH_ERR_ARG, "hh_links_add: records must be 16-byte aligned");
-        for (int64_t off = 0; off < n_rec; off += CH) {
-            const int64_t m = (n_rec - off < CH) ? (n_rec - off) : CH;
-            if (lk->mode != 2) HH_CHECK(links_ensure_capacity(lk, m));
-            HH_CHECK(links_launch_insert(lk, reinterpret_cast<const int4*>(rec) + off, m, stream_offset + off));
-            lk->since_known += m;
-        }
+        HH_CHECK(links_add_chunks(lk, reinterpret_cast<const int4*>(rec), nullptr, n_rec, stream_offset));
     } else {
         if (!lk->d_stage[0]) {
             lk->stage_records = CH;
@@ -1400,13 +1385,11 @@ extern "C" int hh_links_add(hh_links* lk, const int32_t* rec, int64_t n_rec, int
 // bucket is counted in shared memory and the few that a shared-memory table cannot take in a global scratch table;
 // entries are appended to an unordered compact list
 static void links_free_partsets(hh_links* lk) {
-    if (lk->psets) {
-        for (size_t k = 0; k < lk->psets->size(); ++k) {
-            hh_ws_free(lk->ctx, (*lk->psets)[k].buf);
-            hh_dfree((*lk->psets)[k].cursor);
-        }
-        lk->psets->clear();
+    for (hh_partset& ps : lk->psets) {
+        hh_ws_free(lk->ctx, ps.buf);
+        hh_dfree(ps.cursor);
     }
+    lk->psets.clear();
     hh_ws_free(lk->ctx, lk->d_spill);
     hh_dfree(lk->d_spill_cursor);
 }
@@ -1438,7 +1421,6 @@ static uint64_t links_hot_records(int64_t n_used, int bucket_log) {
 // fallback adds its gathered records (16 B each), which take the place of the bucket buffer, and two scratch tables.
 static int links_finish_partitioned(hh_links* lk) {
     hh_ctx* ctx = lk->ctx;
-    const size_t nsets = lk->psets->size();
     unsigned long long c[8];
     HH_CHECK(links_read_counters(lk, c));
     HH_REQUIRE(c[2] == 0, HH_ERR_CAPACITY,
@@ -1477,21 +1459,21 @@ static int links_finish_partitioned(hh_links* lk) {
         HH_CUDA(cudaMemsetAsync(d_agg, 0, 4 * sizeof(unsigned long long), ctx->stream));
         // ---- buckets: records per bucket, dense offsets, every record to its bucket
         const int grid = hh_grid(ctx, 4);
-        for (size_t k = 0; k < nsets; ++k) {
-            const hh_partset& ps = (*lk->psets)[k];
+        for (size_t k = 0; k < lk->psets.size(); ++k) {
+            const hh_partset& ps = lk->psets[k];
             const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
             HH_LAUNCH(ctx, hh_k_part_hist, grid, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
                       k == 0 ? (int64_t)n_spill : 0, blog, d_bcnt);
         }
         HH_CHECK(hh_exclusive_scan_i32(ctx, reinterpret_cast<const int*>(d_bcnt), d_boff, nb));
-        for (size_t k = 0; k < nsets; ++k) {
-            const hh_partset& ps = (*lk->psets)[k];
+        for (size_t k = 0; k < lk->psets.size(); ++k) {
+            const hh_partset& ps = lk->psets[k];
             const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
             HH_LAUNCH(ctx, hh_k_part_scatter2, grid, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
                       k == 0 ? (int64_t)n_spill : 0, blog, d_boff, d_bfill, d_rec2, compact_cap, lk->d_counters);
         }
         links_free_partsets(lk);                               // ordered on the stream behind scatter2
-        HH_CHECK(hh_ws_alloc(ctx, &d_stage_compact, (size_t)compact_cap * 9));
+        HH_CHECK(hh_ws_alloc(ctx, &d_stage_compact, (size_t)compact_cap * HH_E_WORDS));
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 0, 0, sizeof(unsigned long long), ctx->stream));     // entry cursor
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));     // nnz_flank
         // ---- every bucket in shared memory
@@ -1555,9 +1537,9 @@ static int links_finish_partitioned(hh_links* lk) {
                    "hh_links_finish: a bucket of the partitioned counting overflowed (code %llu): set HH_LINKS_PARTITION=0", c[2]);
         lk->nnz = (int64_t)c[0];
         lk->nnz_flank = (int64_t)c[3];
-        HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(lk->nnz > 0 ? lk->nnz : 1) * 9));
+        HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(lk->nnz > 0 ? lk->nnz : 1) * HH_E_WORDS));
         if (lk->nnz)
-            HH_CUDA(cudaMemcpyAsync(lk->d_compact, d_stage_compact, (size_t)lk->nnz * 9 * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+            HH_CUDA(cudaMemcpyAsync(lk->d_compact, d_stage_compact, (size_t)lk->nnz * HH_E_WORDS * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
                                     ctx->stream));
         return HH_OK;
     }();
@@ -1589,70 +1571,87 @@ extern "C" int hh_links_agg_info(hh_links* lk, int64_t* buckets, int64_t* smem_b
     return HH_OK;
 }
 
+// Order array -> entries: dst gets, in array order, the entries that d_order[0..S) names (HH_NONE32 = none): slots of the
+// hash table (keys, vals) or, with keys = NULL, entries of the list passed as `vals`.  Live items per tile, a scan, the
+// gather; the gather from a table also counts the flank entries (counters[3]).
+static int links_compact(hh_links* lk, const uint32_t* d_order, int64_t S, const uint64_t* keys, const hh_slot* vals, uint32_t* dst) {
+    hh_ctx* ctx = lk->ctx;
+    const int64_t nb = (S + HH_CMP_TILE - 1) / HH_CMP_TILE;
+    int* d_bcnt = nullptr;
+    int64_t* d_boff = nullptr;
+    const int rc = [&]() -> int {
+        HH_CHECK(hh_dmalloc(&d_bcnt, (size_t)nb));
+        HH_CHECK(hh_dmalloc(&d_boff, (size_t)nb + 1));
+        HH_LAUNCH(ctx, hh_k_compact_count, (unsigned)nb, 256, 0, d_order, S, d_bcnt);
+        HH_CHECK(hh_exclusive_scan_i32(ctx, d_bcnt, d_boff, (int)nb));
+        HH_LAUNCH(ctx, hh_k_compact_gather, (unsigned)nb, 256, 0, d_order, S, d_boff, keys, vals, dst, lk->d_counters);
+        return HH_OK;
+    }();
+    hh_dfree(d_bcnt);                 // ordered on the stream behind the kernels
+    hh_dfree(d_boff);
+    return rc;
+}
+
+// The direct table becomes the compact list: in dict insertion order (order[first_full] = slot over the whole stream, then
+// compaction), or -- a partition of a routed stream, whose union hh_links_fetch orders lazily -- in slot order.  `who` is
+// the entry point that the error texts name.
+static int links_finish_direct(hh_links* lk, bool ordered, const char* who) {
+    hh_ctx* ctx = lk->ctx;
+    HH_CHECK(links_need_table(lk));
+    unsigned long long c[8];
+    HH_CHECK(links_read_counters(lk, c));
+    HH_REQUIRE(c[2] == 0, HH_ERR_CAPACITY, "%s: hash table overflow (capacity %llu slots)%s", who, (unsigned long long)lk->cap,
+               ordered ? ": pass a larger capacity_hint or use hh_links_add" : "");
+    HH_REQUIRE(c[5] == 0, HH_ERR_ARG,
+               "%s: %llu records have a position outside their contig's bins (e.g. record %llu of the stream)%s", who, c[5], c[6] - 1ull,
+               ordered ? ": positions must lie in [0, contig length)" : "");
+    lk->nnz = (int64_t)c[0];
+    lk->n_used = lk->peer_used + (int64_t)c[1];
+    HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));
+    if (ordered && lk->nnz > 0 && (int64_t)c[4] + 1 > lk->stream_end) lk->stream_end = (int64_t)c[4] + 1;   // merged peers
+    hh_dfree(lk->d_compact);
+    HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(lk->nnz > 0 ? lk->nnz : 1) * HH_E_WORDS));
+    if (lk->nnz > 0) {
+        HH_REQUIRE(ordered || lk->cap <= 0xFFFFFFFFull, HH_ERR_UNSUPPORTED, "%s: table too large", who);
+        const int64_t S = ordered ? lk->stream_end : (int64_t)lk->cap;
+        uint32_t* d_order = nullptr;
+        HH_CHECK(hh_dmalloc(&d_order, (size_t)S));
+        const int rc = [&]() -> int {
+            if (ordered) {
+                HH_CUDA(cudaMemsetAsync(d_order, 0xFF, (size_t)S * sizeof(uint32_t), ctx->stream));
+                HH_LAUNCH(ctx, hh_k_links_scatter_order, hh_grid(ctx, 8), 256, 0, lk->d_keys, lk->d_vals, lk->cap, d_order, S,
+                          lk->d_counters);
+            } else {
+                HH_LAUNCH(ctx, hh_k_links_mark_slots, hh_grid(ctx, 8), 256, 0, lk->d_keys, lk->cap, d_order);
+            }
+            HH_CHECK(links_compact(lk, d_order, S, lk->d_keys, lk->d_vals, lk->d_compact));
+            return links_read_counters(lk, c);
+        }();
+        hh_dfree(d_order);
+        HH_CHECK(rc);
+        HH_REQUIRE(c[2] == 0, HH_ERR_STATE, "%s: first-seen index beyond the stream end (stream_offset misuse)", who);
+        lk->nnz_flank = (int64_t)c[3];
+    }
+    lk->finished = true;
+    lk->ordered = ordered;
+    return HH_OK;
+}
+
+static void links_fill_info(hh_links* lk, hh_links_info* info, int64_t table_slots) {
+    if (!info) return;
+    info->n_records = lk->n_records;
+    info->n_used = lk->n_used;
+    info->nnz_full = lk->nnz;
+    info->nnz_flank = lk->nnz_flank;
+    info->table_slots = table_slots;
+}
+
 extern "C" int hh_links_finish(hh_links* lk, hh_links_info* info) {
     HH_REQUIRE(lk != nullptr, HH_ERR_ARG, "hh_links_finish: NULL handle");
     hh_scope _scope(lk->ctx);
-    hh_ctx* ctx = lk->ctx;
-    HH_CUDA(cudaSetDevice(ctx->device));
-    if (!lk->finished && lk->mode == 2) HH_CHECK(links_finish_partitioned(lk));
-    if (!lk->finished) {
-        HH_CHECK(links_need_table(lk));
-        unsigned long long c[8];
-        HH_CHECK(links_read_counters(lk, c));
-        HH_REQUIRE(c[2] == 0, HH_ERR_CAPACITY,
-                   "hh_links_finish: hash table overflow (capacity %llu slots): pass a larger capacity_hint or use hh_links_add",
-                   (unsigned long long)lk->cap);
-        HH_REQUIRE(c[5] == 0, HH_ERR_ARG,
-                   "hh_links_finish: %llu records have a position outside their contig's bins (e.g. record %llu of the stream): "
-                   "positions must lie in [0, contig length)", c[5], c[6] - 1ull);
-        lk->nnz = (int64_t)c[0];
-        lk->n_used = lk->peer_used + (int64_t)c[1];
-        HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));
-        if (lk->nnz > 0 && (int64_t)c[4] + 1 > lk->stream_end) lk->stream_end = (int64_t)c[4] + 1;   // merged peers
-        const int64_t S = lk->stream_end;
-        hh_dfree(lk->d_compact);
-        HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(lk->nnz > 0 ? lk->nnz : 1) * 9));
-        if (lk->nnz > 0) {
-            uint32_t* d_order = nullptr;
-            int* d_bcnt = nullptr;
-            int64_t* d_boff = nullptr;
-            const int64_t nb = (S + HH_CMP_TILE - 1) / HH_CMP_TILE;
-            int rc = HH_OK;
-            do {
-                if ((rc = hh_dmalloc(&d_order, (size_t)S)) != HH_OK) break;
-                if ((rc = hh_dmalloc(&d_bcnt, (size_t)nb)) != HH_OK) break;
-                if ((rc = hh_dmalloc(&d_boff, (size_t)nb + 1)) != HH_OK) break;
-            } while (0);
-            if (rc == HH_OK) {
-                rc = [&]() -> int {
-                    HH_CUDA(cudaMemsetAsync(d_order, 0xFF, (size_t)S * sizeof(uint32_t), ctx->stream));
-                    HH_LAUNCH(ctx, hh_k_links_scatter_order, hh_grid(ctx, 8), 256, 0, lk->d_keys, lk->d_vals, lk->cap, d_order, S,
-                              lk->d_counters);
-                    HH_LAUNCH(ctx, hh_k_compact_count, (unsigned)nb, 256, 0, d_order, S, d_bcnt);
-                    HH_CHECK(hh_exclusive_scan_i32(ctx, d_bcnt, d_boff, (int)nb));
-                    HH_LAUNCH(ctx, hh_k_compact_gather, (unsigned)nb, 256, 0, d_order, S, d_boff, lk->d_keys, lk->d_vals,
-                              lk->d_compact, lk->d_counters);
-                    HH_CHECK(links_read_counters(lk, c));
-                    return HH_OK;
-                }();
-            }
-            hh_dfree(d_order);
-            hh_dfree(d_bcnt);
-            hh_dfree(d_boff);
-            HH_CHECK(rc);
-            HH_REQUIRE(c[2] == 0, HH_ERR_STATE, "hh_links_finish: first-seen index beyond the stream end (stream_offset misuse)");
-            lk->nnz_flank = (int64_t)c[3];
-        }
-        lk->finished = true;
-        lk->ordered = true;
-    }
-    if (info) {
-        info->n_records = lk->n_records;
-        info->n_used = lk->n_used;
-        info->nnz_full = lk->nnz;
-        info->nnz_flank = lk->nnz_flank;
-        info->table_slots = (int64_t)(lk->mode == 2 ? lk->scap : lk->cap);
-    }
+    HH_CUDA(cudaSetDevice(lk->ctx->device));
+    if (!lk->finished) HH_CHECK(lk->mode == 2 ? links_finish_partitioned(lk) : links_finish_direct(lk, true, "hh_links_finish"));
+    links_fill_info(lk, info, (int64_t)(lk->mode == 2 ? lk->scap : lk->cap));
     return HH_OK;
 }
 
@@ -1660,18 +1659,14 @@ extern "C" int hh_links_finish(hh_links* lk, hh_links_info* info) {
 __global__ void hh_k_links_split(const uint32_t* __restrict__ compact, int64_t nnz, uint32_t* __restrict__ soa, int64_t ht_off) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t* p = compact + e * 9;
-        soa[0 * nnz + e] = p[0];
-        soa[1 * nnz + e] = p[1];
-        soa[2 * nnz + e] = p[2];
-        soa[3 * nnz + e] = p[3];
-        soa[4 * nnz + e] = p[4];
-        soa[5 * nnz + e] = p[5];
+        const uint32_t* p = compact + e * HH_E_WORDS;
+#pragma unroll
+        for (int w = HH_E_I; w <= HH_E_FIRST_FLANK; ++w) soa[w * nnz + e] = p[w];     // the first six words, in entry order
         uint4 h;
-        h.y = p[6];
-        h.z = p[7];
-        h.w = p[8];
-        h.x = p[2] - p[6] - p[7] - p[8];          // HH = full - HT - TH - TT
+        h.y = p[HH_E_HT];
+        h.z = p[HH_E_TH];
+        h.w = p[HH_E_TT];
+        h.x = p[HH_E_FULL] - p[HH_E_HT] - p[HH_E_TH] - p[HH_E_TT];          // HH = full - HT - TH - TT
         reinterpret_cast<uint4*>(soa + ht_off)[e] = h;
     }
 }
@@ -1698,8 +1693,7 @@ extern "C" int hh_links_route(hh_links* lk, const int32_t* rec_dev, int64_t n_re
     int rc = [&]() -> int {
         HH_CUDA(cudaMemsetAsync(d_cnt, 0, 2 * HH_MAX_WORLD * sizeof(unsigned long long), ctx->stream));
         const int contig_mode = lk->d_fbase == nullptr;
-        int64_t blocks = (n_rec + 255) / 256;
-        int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
+        const int grid = links_grid(ctx, n_rec);
         const int4* rec4 = reinterpret_cast<const int4*>(rec_dev);
         HH_LAUNCH(ctx, hh_k_route_count, grid, 256, 0, rec4, n_rec, lk->n_src, contig_mode, world, d_cnt);
         unsigned long long h[HH_MAX_WORLD];
@@ -1735,77 +1729,18 @@ extern "C" int hh_links_add_routed(hh_links* lk, const int32_t* rec_dev, const u
     HH_CUDA(cudaSetDevice(lk->ctx->device));
     HH_REQUIRE(lk->mode != 2, HH_ERR_STATE, "hh_links_add_routed: this table counts a partitioned stream (hh_links_add of a long stream)");
     lk->mode = 1;
-    const int64_t CH = 1ll << 23;
-    for (int64_t off = 0; off < n_rec; off += CH) {
-        const int64_t m = (n_rec - off < CH) ? (n_rec - off) : CH;
-        HH_CHECK(links_ensure_capacity(lk, m));
-        HH_CHECK(links_launch_insert(lk, reinterpret_cast<const int4*>(rec_dev) + off, m, 0, pos_dev + off));
-        lk->since_known += m;
-    }
-    return HH_OK;
+    return links_add_chunks(lk, reinterpret_cast<const int4*>(rec_dev), pos_dev, n_rec, 0);
 }
 
 // compact list of a partition table in slot order (no first-seen ordering: the union is ordered lazily by hh_links_fetch)
 extern "C" int hh_links_finish_partition(hh_links* lk, hh_links_info* info) {
     HH_REQUIRE(lk != nullptr, HH_ERR_ARG, "hh_links_finish_partition: NULL handle");
     hh_scope _scope(lk->ctx);
-    hh_ctx* ctx = lk->ctx;
-    HH_CUDA(cudaSetDevice(ctx->device));
-    if (!lk->finished && lk->mode == 2) HH_CHECK(links_finish_partitioned(lk));     // already an unordered entry list
-    if (!lk->finished) {
-        HH_CHECK(links_need_table(lk));
-        unsigned long long c[8];
-        HH_CHECK(links_read_counters(lk, c));
-        HH_REQUIRE(c[2] == 0, HH_ERR_CAPACITY, "hh_links_finish_partition: hash table overflow (capacity %llu slots)",
-                   (unsigned long long)lk->cap);
-        HH_REQUIRE(c[5] == 0, HH_ERR_ARG,
-                   "hh_links_finish_partition: %llu records have a position outside their contig's bins (e.g. record %llu of the stream)",
-                   c[5], c[6] - 1ull);
-        lk->nnz = (int64_t)c[0];
-        lk->n_used = lk->peer_used + (int64_t)c[1];
-        HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));
-        hh_dfree(lk->d_compact);
-        HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(lk->nnz > 0 ? lk->nnz : 1) * 9));
-        if (lk->nnz > 0) {
-            HH_REQUIRE(lk->cap <= 0xFFFFFFFFull, HH_ERR_UNSUPPORTED, "hh_links_finish_partition: table too large");
-            const int64_t S = (int64_t)lk->cap;
-            uint32_t* d_order = nullptr;
-            int* d_bcnt = nullptr;
-            int64_t* d_boff = nullptr;
-            const int64_t nb = (S + HH_CMP_TILE - 1) / HH_CMP_TILE;
-            int rc = HH_OK;
-            do {
-                if ((rc = hh_dmalloc(&d_order, (size_t)S)) != HH_OK) break;
-                if ((rc = hh_dmalloc(&d_bcnt, (size_t)nb)) != HH_OK) break;
-                if ((rc = hh_dmalloc(&d_boff, (size_t)nb + 1)) != HH_OK) break;
-            } while (0);
-            if (rc == HH_OK) {
-                rc = [&]() -> int {
-                    HH_LAUNCH(ctx, hh_k_links_mark_slots, hh_grid(ctx, 8), 256, 0, lk->d_keys, lk->cap, d_order);
-                    HH_LAUNCH(ctx, hh_k_compact_count, (unsigned)nb, 256, 0, d_order, S, d_bcnt);
-                    HH_CHECK(hh_exclusive_scan_i32(ctx, d_bcnt, d_boff, (int)nb));
-                    HH_LAUNCH(ctx, hh_k_compact_gather, (unsigned)nb, 256, 0, d_order, S, d_boff, lk->d_keys, lk->d_vals,
-                              lk->d_compact, lk->d_counters);
-                    HH_CHECK(links_read_counters(lk, c));
-                    return HH_OK;
-                }();
-            }
-            hh_dfree(d_order);
-            hh_dfree(d_bcnt);
-            hh_dfree(d_boff);
-            HH_CHECK(rc);
-            lk->nnz_flank = (int64_t)c[3];
-        }
-        lk->finished = true;
-        lk->ordered = false;
-    }
-    if (info) {
-        info->n_records = lk->n_records;
-        info->n_used = lk->n_used;
-        info->nnz_full = lk->nnz;
-        info->nnz_flank = lk->nnz_flank;
-        info->table_slots = (int64_t)lk->cap;
-    }
+    HH_CUDA(cudaSetDevice(lk->ctx->device));
+    // a partitioned stream already ends in an unordered entry list
+    if (!lk->finished)
+        HH_CHECK(lk->mode == 2 ? links_finish_partitioned(lk) : links_finish_direct(lk, false, "hh_links_finish_partition"));
+    links_fill_info(lk, info, (int64_t)lk->cap);
     return HH_OK;
 }
 
@@ -1826,13 +1761,12 @@ extern "C" int hh_links_adopt(hh_links* lk, const uint32_t* entries_dev, int64_t
     lk->cap = 0;
     hh_dfree(lk->d_compact);
     lk->d_compact = nullptr;
-    HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(n_entries > 0 ? n_entries : 1) * 9));
+    HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(n_entries > 0 ? n_entries : 1) * HH_E_WORDS));
     HH_CUDA(cudaMemsetAsync(lk->d_counters + 2, 0, 2 * sizeof(unsigned long long), ctx->stream));
     if (n_entries) {
-        HH_CUDA(cudaMemcpyAsync(lk->d_compact, entries_dev, (size_t)n_entries * 9 * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+        HH_CUDA(cudaMemcpyAsync(lk->d_compact, entries_dev, (size_t)n_entries * HH_E_WORDS * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
                                 ctx->stream));
-        int64_t blocks = (n_entries + 255) / 256;
-        int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
+        const int grid = links_grid(ctx, n_entries);
         HH_LAUNCH(ctx, hh_k_list_count_flank, grid, 256, 0, lk->d_compact, n_entries, lk->d_counters);
     }
     HH_CUDA(cudaMemcpyAsync(lk->d_ctg, ctg_links_dev, (size_t)lk->n_ctg * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
@@ -1857,40 +1791,20 @@ static int links_order_list(hh_links* lk) {
     }
     hh_ctx* ctx = lk->ctx;
     const int64_t S = lk->stream_end;
-    const int64_t nb = (S + HH_CMP_TILE - 1) / HH_CMP_TILE;
     uint32_t *d_order = nullptr, *d_sorted = nullptr;
-    int* d_bcnt = nullptr;
-    int64_t* d_boff = nullptr;
-    int rc = HH_OK;
-    do {
-        if ((rc = hh_dmalloc(&d_order, (size_t)S)) != HH_OK) break;
-        if ((rc = hh_dmalloc(&d_sorted, (size_t)lk->nnz * 9)) != HH_OK) break;
-        if ((rc = hh_dmalloc(&d_bcnt, (size_t)nb)) != HH_OK) break;
-        if ((rc = hh_dmalloc(&d_boff, (size_t)nb + 1)) != HH_OK) break;
-    } while (0);
-    unsigned long long c[8] = {0};
-    if (rc == HH_OK) {
-        rc = [&]() -> int {
-            HH_CUDA(cudaMemsetAsync(d_order, 0xFF, (size_t)S * sizeof(uint32_t), ctx->stream));
-            HH_CUDA(cudaMemsetAsync(lk->d_counters + 2, 0, sizeof(unsigned long long), ctx->stream));
-            int64_t blocks = (lk->nnz + 255) / 256;
-            int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
-            HH_LAUNCH(ctx, hh_k_list_scatter_order, grid, 256, 0, lk->d_compact, lk->nnz, d_order, S, lk->d_counters);
-            HH_LAUNCH(ctx, hh_k_compact_count, (unsigned)nb, 256, 0, d_order, S, d_bcnt);
-            HH_CHECK(hh_exclusive_scan_i32(ctx, d_bcnt, d_boff, (int)nb));
-            HH_LAUNCH(ctx, hh_k_compact_gather, (unsigned)nb, 256, 0, d_order, S, d_boff, (const uint64_t*)nullptr,
-                      reinterpret_cast<const hh_slot*>(lk->d_compact), d_sorted, lk->d_counters);
-            HH_CHECK(links_read_counters(lk, c));
-            return HH_OK;
-        }();
-    }
+    const int rc = [&]() -> int {
+        HH_CHECK(hh_dmalloc(&d_order, (size_t)S));
+        HH_CHECK(hh_dmalloc(&d_sorted, (size_t)lk->nnz * HH_E_WORDS));
+        HH_CUDA(cudaMemsetAsync(d_order, 0xFF, (size_t)S * sizeof(uint32_t), ctx->stream));
+        HH_CUDA(cudaMemsetAsync(lk->d_counters + 2, 0, sizeof(unsigned long long), ctx->stream));
+        HH_LAUNCH(ctx, hh_k_list_scatter_order, links_grid(ctx, lk->nnz), 256, 0, lk->d_compact, lk->nnz, d_order, S, lk->d_counters);
+        HH_CHECK(links_compact(lk, d_order, S, nullptr, reinterpret_cast<const hh_slot*>(lk->d_compact), d_sorted));
+        unsigned long long c[8];
+        HH_CHECK(links_read_counters(lk, c));
+        HH_REQUIRE(c[2] == 0, HH_ERR_STATE, "hh_links: first-seen index beyond the stream end (stream_end misuse in hh_links_adopt)");
+        return HH_OK;
+    }();
     hh_dfree(d_order);
-    hh_dfree(d_bcnt);
-    hh_dfree(d_boff);
-    if (rc == HH_OK && c[2] != 0) {
-        hh_dfree(d_sorted);
-        HH_REQUIRE(false, HH_ERR_STATE, "hh_links: first-seen index beyond the stream end (stream_end misuse in hh_links_adopt)");
-    }
     if (rc != HH_OK) {
         hh_dfree(d_sorted);
         return rc;
@@ -1916,8 +1830,7 @@ extern "C" int hh_links_fetch(hh_links* lk, int32_t* key_i, int32_t* key_j, uint
     int rc = [&]() -> int {
         uint32_t* base = d_soa;
         const int64_t ht_off = (6 * nnz + 3) & ~3ll;      // the 4-wide HT block is written with 16-byte stores
-        int64_t blocks = (nnz + 255) / 256;
-        int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
+        const int grid = links_grid(ctx, nnz);
         HH_LAUNCH(ctx, hh_k_links_split, grid, 256, 0, lk->d_compact, nnz, base, ht_off);
         void* dst[6] = {key_i, key_j, full, flank, first_full, first_flank};
         for (int k = 0; k < 6; ++k)
@@ -1944,7 +1857,7 @@ extern "C" int hh_links_export(hh_links* lk, uint32_t* entries_dev, int64_t* ctg
     HH_REQUIRE(lk->finished, HH_ERR_STATE, "hh_links_export: call hh_links_finish first");
     HH_CUDA(cudaSetDevice(lk->ctx->device));
     if (entries_dev && lk->nnz)
-        HH_CUDA(cudaMemcpyAsync(entries_dev, lk->d_compact, (size_t)lk->nnz * 9 * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+        HH_CUDA(cudaMemcpyAsync(entries_dev, lk->d_compact, (size_t)lk->nnz * HH_E_WORDS * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
                                 lk->ctx->stream));
     if (ctg_links_dev)
         HH_CUDA(cudaMemcpyAsync(ctg_links_dev, lk->d_ctg, (size_t)lk->n_ctg * sizeof(int64_t), cudaMemcpyDeviceToDevice,
@@ -1967,8 +1880,7 @@ extern "C" int hh_links_merge(hh_links* lk, const uint32_t* entries_dev, int64_t
     HH_CUDA(cudaSetDevice(ctx->device));
     if (n_entries) {
         HH_CHECK(links_ensure_capacity(lk, n_entries));
-        int64_t blocks = (n_entries + 255) / 256;
-        int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
+        const int grid = links_grid(ctx, n_entries);
         HH_LAUNCH(ctx, hh_k_links_merge, grid, 256, 0, entries_dev, n_entries, lk->d_keys, lk->d_vals, lk->cap, lk->d_counters);
         lk->since_known += n_entries;
     }
@@ -2005,8 +1917,7 @@ extern "C" int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, i
         int* d_nl = reinterpret_cast<int*>(ctx->d_scratch + 8);
         HH_CUDA(cudaMemsetAsync(d_nl, 0, sizeof(int), ctx->stream));
         if (lk->nnz) {
-            int64_t blocks = (lk->nnz + 255) / 256;
-            int grid = (int)(blocks < (int64_t)hh_grid(ctx, 8) ? blocks : (int64_t)hh_grid(ctx, 8));
+            const int grid = links_grid(ctx, lk->nnz);
             HH_LAUNCH(ctx, hh_k_touch, grid, 256, 0, lk->d_compact, lk->nnz, lk->d_keep, lk->d_ctg, normalize_by_nlinks,
                       hh_links_hap_dev(lk), w, d_touch);
         }
@@ -2052,7 +1963,6 @@ extern "C" int hh_links_destroy(hh_links* lk) {
     hh_dfree(lk->d_keep);
     hh_dfree(lk->d_hap);
     links_free_partsets(lk);
-    delete lk->psets;
     delete lk;
     return HH_OK;
 }

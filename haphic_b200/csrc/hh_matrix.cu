@@ -30,9 +30,9 @@ __global__ void hh_k_mat_count(const uint32_t* __restrict__ compact, int64_t nnz
                                double w, int* __restrict__ colcnt) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t* p = compact + e * 9;
-        if (p[3] == 0) continue;
-        const int ii = index[p[0]], jj = index[p[1]];
+        const uint32_t* p = compact + e * HH_E_WORDS;
+        if (p[HH_E_FLANK] == 0) continue;
+        const int ii = index[p[HH_E_I]], jj = index[p[HH_E_J]];
         if (ii < 0 || jj < 0) continue;                 // 329-330
         double x;
         if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
@@ -52,9 +52,9 @@ __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t n
                                  int32_t* __restrict__ row, float* __restrict__ val) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t* p = compact + e * 9;
-        if (p[3] == 0) continue;
-        const int ii = index[p[0]], jj = index[p[1]];
+        const uint32_t* p = compact + e * HH_E_WORDS;
+        if (p[HH_E_FLANK] == 0) continue;
+        const int ii = index[p[HH_E_I]], jj = index[p[HH_E_J]];
         if (ii < 0 || jj < 0) continue;
         double x;
         if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
