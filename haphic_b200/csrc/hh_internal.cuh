@@ -20,8 +20,8 @@ enum { HH_E_I, HH_E_J, HH_E_FULL, HH_E_FLANK, HH_E_FIRST_FULL, HH_E_FIRST_FLANK,
 // How the matrix sees one entry of the compact link table: the flank count, or
 // links / (tot_i * tot_j) ** 0.5 in fp64 with normalize (normalize_by_nlinks, 718-724), then -- when hap != NULL and the
 // two ends lie on different haplotypes -- x - x * w with two roundings (reduce_inter_hap_HiC_links, 695-707).  Returns
-// false when the entry is not in the (reduced) flank_link_dict: no flank link, or reduced to exactly 0.  hh_k_touch,
-// hh_k_mat_count and hh_k_mat_scatter all decide through this one function, so pattern, values and first-seen indices
+// false when the entry is not in the (reduced) flank_link_dict: no flank link, or reduced to exactly 0.  hh_k_touch
+// and hh_k_mat_scatter both decide through this one function, so pattern, values and first-seen indices
 // cannot disagree.
 __device__ __forceinline__ bool hh_flank_value(const uint32_t* __restrict__ p, const unsigned long long* __restrict__ ctg_tot,
                                                int normalize, const int32_t* __restrict__ hap, double w, double* x_out) {
@@ -44,7 +44,8 @@ int32_t hh_links_n_ctg(hh_links* lk);
 hh_ctx* hh_links_ctx(hh_links* lk);
 const uint32_t* hh_links_compact(hh_links* lk, int64_t* nnz);
 const unsigned long long* hh_links_ctg_totals(hh_links* lk);
-int32_t* hh_links_index_dev(hh_links* lk, int32_t* n_linked);
+const int32_t* hh_links_index_dev(hh_links* lk, int32_t* n_linked);   // the table's copy: hh_matrix_from_links never writes it
+const int32_t* hh_links_degree_dev(hh_links* lk, int64_t* n_pass);   // per-fragment degree and passing entries of that index
 uint8_t* hh_links_keep_dev(hh_links* lk);
 bool hh_links_finished(hh_links* lk);
 const int32_t* hh_links_hap_dev(hh_links* lk);   // haplotypes of the last phased hh_links_linked_index_phased; NULL = none

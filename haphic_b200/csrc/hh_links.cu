@@ -16,6 +16,7 @@
 // compaction (no sort): order[first_full] = slot, then compact.
 #include "hh_common.cuh"
 #include "hh_internal.cuh"
+#include <cub/cub.cuh>
 #include <stdlib.h>
 #include <algorithm>
 #include <vector>
@@ -80,6 +81,16 @@ struct hh_links {
     uint8_t* d_keep;
     int32_t* d_hap;                  // [n_ctg] haplotype of every fragment (allocated on the first phased call)
     bool phased;                     // the last hh_links_linked_index_phased got a haplotype array
+    int32_t* d_deg;                  // [n_ctg] entries of the (reduced) flank dict that touch each kept fragment
+    int64_t n_pass;                  // entries of that dict between kept fragments: the matrix has 2 n_pass off-diagonal entries
+    // what d_index / d_deg / n_pass were computed from: the index is reused while all of it is unchanged
+    uint64_t gen;                    // bumped whenever d_compact or d_ctg is rewritten (finish, adopt, merge)
+    bool ix_valid;
+    uint64_t ix_gen;
+    int ix_normalize;
+    double ix_w;
+    std::vector<uint8_t> ix_keep;
+    std::vector<int32_t> ix_hap;     // empty: unphased
 };
 
 __device__ __forceinline__ uint64_t hh_mix64(uint64_t k) {
@@ -1013,9 +1024,14 @@ hh_k_compact_gather(const uint32_t* __restrict__ order, int64_t n, const int64_t
 // dict_to_matrix index assignment (327-349): first touch of each fragment in flank-dict order.  An entry that the
 // phasing reduction deleted is not in the dict and touches nothing.
 // ---------------------------------------------------------------------------------------------
-__global__ void hh_k_touch(const uint32_t* __restrict__ compact, int64_t nnz, const uint8_t* __restrict__ keep,
-                           const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
-                           double w, unsigned long long* __restrict__ touch) {
+__global__ void __launch_bounds__(256)
+hh_k_touch(const uint32_t* __restrict__ compact, int64_t nnz, const uint8_t* __restrict__ keep,
+           const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap, double w,
+           unsigned long long* __restrict__ touch, int* __restrict__ deg, unsigned long long* __restrict__ n_pass) {
+    __shared__ unsigned int s_pass;
+    if (threadIdx.x == 0) s_pass = 0;
+    __syncthreads();
+    unsigned int my_pass = 0;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
         const uint32_t* p = compact + e * HH_E_WORDS;
@@ -1025,31 +1041,33 @@ __global__ void hh_k_touch(const uint32_t* __restrict__ compact, int64_t nnz, co
         double x;
         if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;   // not in flank_link_dict
         const unsigned long long t = (unsigned long long)p[HH_E_FIRST_FLANK] * 2ull;
-        atomicMin(touch + i, t);
-        atomicMin(touch + j, t + 1ull);
+        // touch values only fall, so a value read from L2 that is already below t makes the atomic a no-op; most are
+        if (t < __ldcg(touch + i)) atomicMin(touch + i, t);
+        if (t + 1ull < __ldcg(touch + j)) atomicMin(touch + j, t + 1ull);
+        atomicAdd(deg + i, 1);                          // the column counts of the matrix (hh_matrix_from_links_phased)
+        atomicAdd(deg + j, 1);
+        my_pass++;
     }
+    my_pass = (unsigned)hh_warp_sum((int)my_pass);
+    if ((threadIdx.x & 31) == 0 && my_pass) atomicAdd(&s_pass, my_pass);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_pass) atomicAdd(n_pass, (unsigned long long)s_pass);
 }
 
-// index[c] = number of touched fragments touched earlier than c (touch values are unique)
-__global__ void __launch_bounds__(256)
-hh_k_rank_touch(const unsigned long long* __restrict__ touch, int n, int32_t* __restrict__ index, int* __restrict__ n_linked) {
-    __shared__ unsigned long long tile[1024];
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned long long mine = (c < n) ? touch[c] : ~0ull;
-    int rank = 0;
-    for (int base = 0; base < n; base += 1024) {
-        for (int k = threadIdx.x; k < 1024; k += blockDim.x) tile[k] = (base + k < n) ? touch[base + k] : ~0ull;
-        __syncthreads();
-        if (mine != ~0ull) {
-#pragma unroll 8
-            for (int k = 0; k < 1024; ++k) rank += (tile[k] < mine) ? 1 : 0;
-        }
-        __syncthreads();
-    }
-    if (c < n) {
-        index[c] = (mine != ~0ull) ? rank : -1;
-        if (mine != ~0ull) atomicAdd(n_linked, 1);
-    }
+__global__ void hh_k_iota_i32(int32_t* __restrict__ p, int n) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) p[k] = k;
+}
+
+// After the (touch, fragment) pairs are sorted by touch: index[fragment] = its rank among the touched ones, -1 for the
+// untouched (touch values are unique; the untouched sort last); out[0] = number touched
+__global__ void hh_k_rank_sorted(const unsigned long long* __restrict__ touch_sorted, const int32_t* __restrict__ frag_sorted, int n,
+                                 int32_t* __restrict__ index, unsigned long long* __restrict__ out) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const bool touched = touch_sorted[k] != ~0ull;
+    index[frag_sorted[k]] = touched ? k : -1;
+    if (touched && (k == n - 1 || touch_sorted[k + 1] == ~0ull)) out[0] = (unsigned long long)(k + 1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1147,6 +1165,7 @@ static int links_create_common(hh_ctx* ctx, int32_t n_key, const int64_t* key_le
         if ((rc = hh_dmalloc(&lk->d_counters, 8)) != HH_OK) break;
         if ((rc = hh_dmalloc(&lk->d_index, n_key)) != HH_OK) break;
         if ((rc = hh_dmalloc(&lk->d_keep, n_key)) != HH_OK) break;
+        if ((rc = hh_dmalloc(&lk->d_deg, n_key)) != HH_OK) break;
         if (frag_base) {
             if ((rc = hh_dmalloc(&lk->d_src_rank, n_src)) != HH_OK) break;
             if ((rc = hh_dmalloc(&lk->d_fbase, (size_t)n_src + 1)) != HH_OK) break;
@@ -1559,6 +1578,7 @@ static int links_finish_partitioned(hh_links* lk) {
     links_free_partsets(lk);
     HH_CHECK(rc);
     lk->finished = true;
+    lk->gen++;                  // the linked index of an earlier table does not apply
     lk->ordered = false;        // dict insertion order is restored by the first hh_links_fetch (links_order_list)
     return HH_OK;
 }
@@ -1633,6 +1653,7 @@ static int links_finish_direct(hh_links* lk, bool ordered, const char* who) {
         lk->nnz_flank = (int64_t)c[3];
     }
     lk->finished = true;
+    lk->gen++;                  // the linked index of an earlier table does not apply
     lk->ordered = ordered;
     return HH_OK;
 }
@@ -1761,6 +1782,7 @@ extern "C" int hh_links_adopt(hh_links* lk, const uint32_t* entries_dev, int64_t
     lk->cap = 0;
     hh_dfree(lk->d_compact);
     lk->d_compact = nullptr;
+    lk->gen++;                  // the linked index of the old list does not apply, even if this call fails
     HH_CHECK(hh_dmalloc(&lk->d_compact, (size_t)(n_entries > 0 ? n_entries : 1) * HH_E_WORDS));
     HH_CUDA(cudaMemsetAsync(lk->d_counters + 2, 0, 2 * sizeof(unsigned long long), ctx->stream));
     if (n_entries) {
@@ -1875,6 +1897,7 @@ extern "C" int hh_links_merge(hh_links* lk, const uint32_t* entries_dev, int64_t
     lk->mode = 1;
     HH_CHECK(links_need_table(lk));
     lk->finished = false;   // a finished table is re-opened: the next hh_links_finish rebuilds the ordered view
+    lk->gen++;
     HH_REQUIRE(n_entries >= 0 && (entries_dev || n_entries == 0), HH_ERR_ARG, "hh_links_merge: bad entries");
     hh_ctx* ctx = lk->ctx;
     HH_CUDA(cudaSetDevice(ctx->device));
@@ -1896,6 +1919,16 @@ extern "C" int hh_links_linked_index(hh_links* lk, const uint8_t* keep, int32_t*
     return hh_links_linked_index_phased(lk, keep, 0, nullptr, 0.0, index, n_linked);
 }
 
+// The index, the degrees and the passing count depend on the table and on (keep, hap, w, normalize_by_nlinks) only.  They
+// are kept with what they were computed from, and a call with the same table generation and the same array contents
+// reuses them: bench.py, `haphic cluster` and dist.py call linked_index and then to_matrix with the same arguments.
+static bool links_index_current(const hh_links* lk, const uint8_t* keep, int normalize, const int32_t* hap, double w) {
+    if (!lk->ix_valid || lk->ix_gen != lk->gen || lk->ix_normalize != normalize) return false;
+    if ((hap != nullptr) != !lk->ix_hap.empty()) return false;
+    if (hap && (lk->ix_w != w || memcmp(hap, lk->ix_hap.data(), (size_t)lk->n_ctg * sizeof(int32_t)) != 0)) return false;
+    return memcmp(keep, lk->ix_keep.data(), (size_t)lk->n_ctg) == 0;
+}
+
 extern "C" int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, int normalize_by_nlinks, const int32_t* hap,
                                             double w, int32_t* index, int32_t* n_linked) {
     HH_REQUIRE(lk && keep, HH_ERR_ARG, "hh_links_linked_index: NULL argument");
@@ -1904,33 +1937,63 @@ extern "C" int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, i
     HH_REQUIRE(!hap || (w >= 0.0 && w <= 1.0), HH_ERR_ARG, "hh_links_linked_index_phased: phasing weight %g outside [0, 1]", w);
     hh_ctx* ctx = lk->ctx;
     HH_CUDA(cudaSetDevice(ctx->device));
-    lk->phased = hap != nullptr;
-    if (hap) {
-        if (!lk->d_hap) HH_CHECK(hh_dmalloc(&lk->d_hap, (size_t)lk->n_ctg));
-        HH_CUDA(cudaMemcpyAsync(lk->d_hap, hap, (size_t)lk->n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    }
-    unsigned long long* d_touch = nullptr;
-    HH_CHECK(hh_dmalloc(&d_touch, (size_t)lk->n_ctg));
-    int rc = [&]() -> int {
-        HH_CUDA(cudaMemcpyAsync(lk->d_keep, keep, (size_t)lk->n_ctg, cudaMemcpyHostToDevice, ctx->stream));
-        HH_CUDA(cudaMemsetAsync(d_touch, 0xFF, (size_t)lk->n_ctg * sizeof(unsigned long long), ctx->stream));
-        int* d_nl = reinterpret_cast<int*>(ctx->d_scratch + 8);
-        HH_CUDA(cudaMemsetAsync(d_nl, 0, sizeof(int), ctx->stream));
-        if (lk->nnz) {
-            const int grid = links_grid(ctx, lk->nnz);
-            HH_LAUNCH(ctx, hh_k_touch, grid, 256, 0, lk->d_compact, lk->nnz, lk->d_keep, lk->d_ctg, normalize_by_nlinks,
-                      hh_links_hap_dev(lk), w, d_touch);
+    const int n_ctg = lk->n_ctg;
+    if (!links_index_current(lk, keep, normalize_by_nlinks, hap, w)) {
+        lk->ix_valid = false;
+        lk->phased = hap != nullptr;
+        if (hap) {
+            if (!lk->d_hap) HH_CHECK(hh_dmalloc(&lk->d_hap, (size_t)n_ctg));
+            HH_CUDA(cudaMemcpyAsync(lk->d_hap, hap, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
         }
-        HH_LAUNCH(ctx, hh_k_rank_touch, (lk->n_ctg + 255) / 256, 256, 0, d_touch, lk->n_ctg, lk->d_index, d_nl);
-        HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 8, d_nl, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        if (index)
-            HH_CUDA(cudaMemcpyAsync(index, lk->d_index, (size_t)lk->n_ctg * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+        unsigned long long *d_touch = nullptr, *d_touch_sorted = nullptr;
+        int32_t *d_frag = nullptr, *d_frag_sorted = nullptr;
+        uint8_t* d_tmp = nullptr;
+        int rc = [&]() -> int {
+            HH_CHECK(hh_dmalloc(&d_touch, (size_t)n_ctg * 2));
+            HH_CHECK(hh_dmalloc(&d_frag, (size_t)n_ctg * 2));
+            d_touch_sorted = d_touch + n_ctg;
+            d_frag_sorted = d_frag + n_ctg;
+            // touch values are below 2^33 and the untouched ones (all bits set) are 2^34 - 1 in the low 34 bits
+            size_t tmp_bytes = 0;
+            HH_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_touch, d_touch_sorted, d_frag, d_frag_sorted, n_ctg, 0, 34,
+                                                    ctx->stream));
+            HH_CHECK(hh_dmalloc(&d_tmp, tmp_bytes));
+            HH_CUDA(cudaMemcpyAsync(lk->d_keep, keep, (size_t)n_ctg, cudaMemcpyHostToDevice, ctx->stream));
+            HH_CUDA(cudaMemsetAsync(d_touch, 0xFF, (size_t)n_ctg * sizeof(unsigned long long), ctx->stream));
+            HH_CUDA(cudaMemsetAsync(lk->d_deg, 0, (size_t)n_ctg * sizeof(int32_t), ctx->stream));
+            unsigned long long* d_out = reinterpret_cast<unsigned long long*>(ctx->d_scratch + 8);   // [0] touched  [1] passing
+            HH_CUDA(cudaMemsetAsync(d_out, 0, 2 * sizeof(unsigned long long), ctx->stream));
+            if (lk->nnz) {
+                const int grid = links_grid(ctx, lk->nnz);
+                HH_LAUNCH(ctx, hh_k_touch, grid, 256, 0, lk->d_compact, lk->nnz, lk->d_keep, lk->d_ctg, normalize_by_nlinks,
+                          hh_links_hap_dev(lk), w, d_touch, lk->d_deg, d_out + 1);
+            }
+            HH_LAUNCH(ctx, hh_k_iota_i32, (n_ctg + 255) / 256, 256, 0, d_frag, n_ctg);
+            HH_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_touch, d_touch_sorted, d_frag, d_frag_sorted, n_ctg, 0, 34,
+                                                    ctx->stream));
+            HH_LAUNCH(ctx, hh_k_rank_sorted, (n_ctg + 255) / 256, 256, 0, d_touch_sorted, d_frag_sorted, n_ctg, lk->d_index, d_out);
+            HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 8, d_out, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+            HH_CUDA(cudaStreamSynchronize(ctx->stream));
+            lk->n_linked = (int32_t)ctx->h_scratch[8];
+            lk->n_pass = (int64_t)ctx->h_scratch[9];
+            return HH_OK;
+        }();
+        hh_dfree(d_touch);
+        hh_dfree(d_frag);
+        hh_dfree(d_tmp);
+        HH_CHECK(rc);
+        lk->ix_keep.assign(keep, keep + n_ctg);
+        if (hap) lk->ix_hap.assign(hap, hap + n_ctg);
+        else lk->ix_hap.clear();
+        lk->ix_w = w;
+        lk->ix_normalize = normalize_by_nlinks;
+        lk->ix_gen = lk->gen;
+        lk->ix_valid = true;
+    }
+    if (index) {
+        HH_CUDA(cudaMemcpyAsync(index, lk->d_index, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaStreamSynchronize(ctx->stream));
-        lk->n_linked = *reinterpret_cast<int*>(ctx->h_scratch + 8);
-        return HH_OK;
-    }();
-    hh_dfree(d_touch);
-    HH_CHECK(rc);
+    }
     if (n_linked) *n_linked = lk->n_linked;
     return HH_OK;
 }
@@ -1962,6 +2025,7 @@ extern "C" int hh_links_destroy(hh_links* lk) {
     hh_dfree(lk->d_index);
     hh_dfree(lk->d_keep);
     hh_dfree(lk->d_hap);
+    hh_dfree(lk->d_deg);
     links_free_partsets(lk);
     delete lk;
     return HH_OK;
@@ -1972,7 +2036,8 @@ int32_t hh_links_n_ctg(hh_links* lk) { return lk->n_ctg; }
 hh_ctx* hh_links_ctx(hh_links* lk) { return lk->ctx; }
 const uint32_t* hh_links_compact(hh_links* lk, int64_t* nnz) { *nnz = lk->nnz; return lk->d_compact; }
 const unsigned long long* hh_links_ctg_totals(hh_links* lk) { return lk->d_ctg; }
-int32_t* hh_links_index_dev(hh_links* lk, int32_t* n_linked) { *n_linked = lk->n_linked; return lk->d_index; }
+const int32_t* hh_links_index_dev(hh_links* lk, int32_t* n_linked) { *n_linked = lk->n_linked; return lk->d_index; }
+const int32_t* hh_links_degree_dev(hh_links* lk, int64_t* n_pass) { *n_pass = lk->n_pass; return lk->d_deg; }
 uint8_t* hh_links_keep_dev(hh_links* lk) { return lk->d_keep; }
 bool hh_links_finished(hh_links* lk) { return lk->finished; }
 const int32_t* hh_links_hap_dev(hh_links* lk) { return lk->phased ? lk->d_hap : nullptr; }

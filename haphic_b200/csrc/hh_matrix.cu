@@ -3,6 +3,7 @@
 // inter-haplotype entries are reduced first (reduce_inter_hap_HiC_links, 695-707; hh_flank_value).
 #include "hh_common.cuh"
 #include "hh_internal.cuh"
+#include <algorithm>
 
 __global__ void hh_k_set_tail(const int32_t* __restrict__ tail, int n_tail, int n_linked, const uint8_t* __restrict__ keep,
                               int32_t* __restrict__ index, int n_ctg, int* __restrict__ err) {
@@ -25,27 +26,31 @@ __global__ void hh_k_check_index(const int32_t* __restrict__ index, const uint8_
     if (keep[c] ? (ix < 0 || ix >= n) : (ix >= 0)) atomicExch(err, 2);
 }
 
-__global__ void hh_k_mat_count(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
-                               const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
-                               double w, int* __restrict__ colcnt) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t* p = compact + e * HH_E_WORDS;
-        if (p[HH_E_FLANK] == 0) continue;
-        const int ii = index[p[HH_E_I]], jj = index[p[HH_E_J]];
-        if (ii < 0 || jj < 0) continue;                 // 329-330
-        double x;
-        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
-        atomicAdd(colcnt + ii, 1);
-        atomicAdd(colcnt + jj, 1);
-    }
-}
-
 __global__ void hh_k_fill_i32(int* __restrict__ p, int v, int n) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
 }
 
+// column counts from the degrees the index pass accumulated: a linked fragment's column holds its entries and the self
+// loop; the tail columns keep the self loop the fill gave them
+__global__ void hh_k_mat_colcnt(const int32_t* __restrict__ index, const int32_t* __restrict__ deg, int n_ctg, int self_loop,
+                                int* __restrict__ colcnt) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_ctg) return;
+    const int ix = index[c];
+    if (ix >= 0) colcnt[ix] = deg[c] + self_loop;
+}
+
+// Each self loop takes slot 0 of its column (362-364); the cursors start at 1, so no atomic is needed here
+__global__ void hh_k_mat_self_loops(int n, const int64_t* __restrict__ colptr, int32_t* __restrict__ row, float* __restrict__ val) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    const int64_t q = colptr[c];
+    row[q] = c;
+    val[q] = 1.0f;
+}
+
+// every passing entry to its two columns; the order of rows inside a column is left unspecified
 __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
                                  const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
                                  double w, const int64_t* __restrict__ colptr, int* __restrict__ cursor,
@@ -55,7 +60,7 @@ __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t n
         const uint32_t* p = compact + e * HH_E_WORDS;
         if (p[HH_E_FLANK] == 0) continue;
         const int ii = index[p[HH_E_I]], jj = index[p[HH_E_J]];
-        if (ii < 0 || jj < 0) continue;
+        if (ii < 0 || jj < 0) continue;                 // 329-330
         double x;
         if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
         const float v = (float)x;                      // coo_matrix(dtype=float32) (368)
@@ -66,15 +71,6 @@ __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t n
         row[q] = jj;
         val[q] = v;
     }
-}
-
-__global__ void hh_k_mat_diag(int n, const int64_t* __restrict__ colptr, int* __restrict__ cursor, int32_t* __restrict__ row,
-                              float* __restrict__ val) {
-    int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= n) return;
-    const int64_t q = colptr[c] + atomicAdd(cursor + c, 1);     // self loops = 1 (362-364)
-    row[q] = c;
-    val[q] = 1.0f;
 }
 
 static int matrix_alloc(hh_ctx* ctx, int32_t n, int64_t nnz, hh_matrix** out) {
@@ -110,66 +106,62 @@ extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, co
     hh_ctx* ctx = hh_links_ctx(lk);
     HH_CUDA(cudaSetDevice(ctx->device));
     const int n_ctg = hh_links_n_ctg(lk);
-    // (re)compute the first-seen indices for this keep mask
+    // the first-seen indices, degrees and passing count for this keep mask: reused when hh_links_linked_index_phased
+    // computed them from the same arguments, recomputed (with one sync) otherwise
     int32_t n_linked = 0;
     HH_CHECK(hh_links_linked_index_phased(lk, keep, normalize_by_nlinks, hap, w, nullptr, &n_linked));
     const int32_t* d_hap = hh_links_hap_dev(lk);
-    int32_t* d_index = hh_links_index_dev(lk, &n_linked);
+    const int32_t* d_index = hh_links_index_dev(lk, &n_linked);
+    int64_t n_pass = 0;
+    const int32_t* d_deg = hh_links_degree_dev(lk, &n_pass);
     const uint8_t* d_keep = hh_links_keep_dev(lk);
+    // a tail longer than the unlinked fragments must repeat or list a linked / absent id: refused before the matrix is sized
+    HH_REQUIRE(n_tail <= n_ctg - n_linked, HH_ERR_ARG,
+               "hh_matrix_from_links: tail lists an id that is dropped, linked, repeated or out of range");
     const int n = n_linked + n_tail;
     HH_REQUIRE(n > 0, HH_ERR_ARG, "hh_matrix_from_links: empty fragment set");
-    int* d_err = reinterpret_cast<int*>(ctx->d_scratch + 9);
-    HH_CUDA(cudaMemsetAsync(d_err, 0, sizeof(int), ctx->stream));
+    const int sl = add_self_loops ? 1 : 0;
+    const int64_t nnz = 2 * n_pass + (int64_t)sl * n;      // known before any sync: the matrix is allocated up front
+    int* d_err = reinterpret_cast<int*>(ctx->d_scratch + 10);
     int32_t* d_tail = nullptr;
     int* d_cnt = nullptr;
-    int* d_cursor = nullptr;
     hh_matrix* m = nullptr;
     int rc = [&]() -> int {
+        HH_CHECK(matrix_alloc(ctx, n, nnz, &m));
+        // the matrix gets its own copy of the index, and the tail goes there: the table's index stays reusable
+        HH_CHECK(hh_dmalloc(&m->d_index, (size_t)n_ctg));
+        m->n_index = n_ctg;
+        HH_CUDA(cudaMemcpyAsync(m->d_index, d_index, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
+        HH_CUDA(cudaMemsetAsync(d_err, 0, sizeof(int), ctx->stream));
         if (n_tail) {
             HH_CHECK(hh_dmalloc(&d_tail, (size_t)n_tail));
             HH_CUDA(cudaMemcpyAsync(d_tail, tail, (size_t)n_tail * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-            HH_LAUNCH(ctx, hh_k_set_tail, (n_tail + 255) / 256, 256, 0, d_tail, n_tail, n_linked, d_keep, d_index, n_ctg, d_err);
+            HH_LAUNCH(ctx, hh_k_set_tail, (n_tail + 255) / 256, 256, 0, d_tail, n_tail, n_linked, d_keep, m->d_index, n_ctg, d_err);
         }
-        HH_LAUNCH(ctx, hh_k_check_index, (n_ctg + 255) / 256, 256, 0, d_index, d_keep, n_ctg, n, d_err);
+        HH_LAUNCH(ctx, hh_k_check_index, (n_ctg + 255) / 256, 256, 0, m->d_index, d_keep, n_ctg, n, d_err);
         HH_CHECK(hh_dmalloc(&d_cnt, (size_t)n));
-        HH_CHECK(hh_dmalloc(&d_cursor, (size_t)n));
-        HH_LAUNCH(ctx, hh_k_fill_i32, (n + 255) / 256, 256, 0, d_cnt, add_self_loops ? 1 : 0, n);     // the self loop
-        HH_CUDA(cudaMemsetAsync(d_cursor, 0, (size_t)n * sizeof(int), ctx->stream));
+        HH_LAUNCH(ctx, hh_k_fill_i32, (n + 255) / 256, 256, 0, d_cnt, sl, n);
+        HH_LAUNCH(ctx, hh_k_mat_colcnt, (n_ctg + 255) / 256, 256, 0, d_index, d_deg, n_ctg, sl, d_cnt);
+        HH_CHECK(hh_exclusive_scan_i32(ctx, d_cnt, m->d_colptr, n));
+        int* d_cursor = d_cnt;                             // the counts are scanned: the buffer becomes the column cursors
+        HH_LAUNCH(ctx, hh_k_fill_i32, (n + 255) / 256, 256, 0, d_cursor, sl, n);
+        if (sl) HH_LAUNCH(ctx, hh_k_mat_self_loops, (n + 255) / 256, 256, 0, n, m->d_colptr, m->d_row, m->d_val);
         int64_t nnz_c = 0;
         const uint32_t* compact = hh_links_compact(lk, &nnz_c);
-        const int gridc = (int)((nnz_c + 255) / 256 < (int64_t)ctx->sm_count * 8 ? (nnz_c + 255) / 256 : (int64_t)ctx->sm_count * 8);
-        if (nnz_c) HH_LAUNCH(ctx, hh_k_mat_count, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk),
-                              normalize_by_nlinks, d_hap, w, d_cnt);
-        int64_t* d_ptr = nullptr;
-        HH_CHECK(hh_dmalloc(&d_ptr, (size_t)n + 1));
-        int rc2 = [&]() -> int {
-            HH_CHECK(hh_exclusive_scan_i32(ctx, d_cnt, d_ptr, n));
-            HH_CUDA(cudaMemcpyAsync(ctx->h_scratch, d_ptr + n, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-            HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 1, d_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-            HH_CUDA(cudaStreamSynchronize(ctx->stream));
-            const int err = *reinterpret_cast<int*>(ctx->h_scratch + 1);
-            HH_REQUIRE(err == 0, HH_ERR_ARG,
-                       err == 1 ? "hh_matrix_from_links: tail lists an id that is dropped, linked, repeated or out of range"
-                                : "hh_matrix_from_links: keep mask and tail do not cover the fragment set exactly");
-            const int64_t nnz = (int64_t)ctx->h_scratch[0];
-            HH_CHECK(matrix_alloc(ctx, n, nnz, &m));
-            HH_CUDA(cudaMemcpyAsync(m->d_colptr, d_ptr, ((size_t)n + 1) * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-            if (nnz_c)
-                HH_LAUNCH(ctx, hh_k_mat_scatter, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks,
-                          d_hap, w, m->d_colptr, d_cursor, m->d_row, m->d_val);
-            if (add_self_loops) HH_LAUNCH(ctx, hh_k_mat_diag, (n + 255) / 256, 256, 0, n, m->d_colptr, d_cursor, m->d_row, m->d_val);
-            HH_CHECK(hh_dmalloc(&m->d_index, (size_t)n_ctg));
-            m->n_index = n_ctg;
-            HH_CUDA(cudaMemcpyAsync(m->d_index, d_index, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyDeviceToDevice, ctx->stream));
-            HH_CUDA(cudaStreamSynchronize(ctx->stream));
-            return HH_OK;
-        }();
-        hh_dfree(d_ptr);
-        return rc2;
+        const int gridc = (int)std::min<int64_t>((nnz_c + 255) / 256, (int64_t)ctx->sm_count * 8);
+        if (n_pass)
+            HH_LAUNCH(ctx, hh_k_mat_scatter, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks, d_hap,
+                      w, m->d_colptr, d_cursor, m->d_row, m->d_val);
+        HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 10, d_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaStreamSynchronize(ctx->stream));
+        const int err = *reinterpret_cast<int*>(ctx->h_scratch + 10);
+        HH_REQUIRE(err == 0, HH_ERR_ARG,
+                   err == 1 ? "hh_matrix_from_links: tail lists an id that is dropped, linked, repeated or out of range"
+                            : "hh_matrix_from_links: keep mask and tail do not cover the fragment set exactly");
+        return HH_OK;
     }();
     hh_dfree(d_tail);
     hh_dfree(d_cnt);
-    hh_dfree(d_cursor);
     if (rc != HH_OK) {
         hh_matrix_destroy(m);
         return rc;
