@@ -176,6 +176,17 @@ __device__ __forceinline__ float4 hh_ld_stream_f4(const float4* p) {
     return r;
 }
 
+// CTAs of `kernel` (at `threads` threads and `smem` bytes of dynamic shared memory) that the GPU holds at once: the grid of
+// a persistent kernel whose CTAs each loop over a fixed share of the work, so that none waits for another to exit
+template <typename K>
+static inline int hh_resident_grid(hh_ctx* ctx, K kernel, int threads, size_t smem, int* grid) {
+    int per_sm = 0;
+    HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+    HH_REQUIRE(per_sm > 0, HH_ERR_CUDA, "a kernel of %d threads and %zu bytes of shared memory does not fit an SM", threads, smem);
+    *grid = ctx->sm_count * per_sm;
+    return HH_OK;
+}
+
 // single-CTA exclusive scan of n ints (n up to a few million): out[i] = sum_{k<i} in[k], out[n] = total
 __global__ void hh_k_scan_small(const int* __restrict__ in, int64_t* __restrict__ out, int n);
 // multi-block stream compaction support

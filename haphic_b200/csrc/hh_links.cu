@@ -1298,8 +1298,9 @@ static int links_launch_insert(hh_links* lk, const int4* d_rec, int64_t n_rec, i
     hh_ctx* ctx = lk->ctx;
     if (lk->mode == 2 && d_pos == nullptr) {
         const int64_t tiles = (n_rec + HH_PART_TILE - 1) / HH_PART_TILE;
-        int grid = (int)(tiles < (int64_t)hh_grid(ctx, 3) ? tiles : (int64_t)hh_grid(ctx, 3));
-        if (grid < 1) grid = 1;
+        int grid = 0;
+        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter, 512, 0, &grid));
+        grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, grid));
         const hh_partset& ps = lk->psets.back();
         HH_LAUNCH(ctx, hh_k_part_scatter, grid, 512, 0, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank, lk->d_nx,
                   lk->flank_bp, lk->npart_log, ps.buf, ps.pcap, ps.cursor, lk->d_spill, lk->spill_cap, lk->d_spill_cursor,
@@ -1477,7 +1478,9 @@ static int links_finish_partitioned(hh_links* lk) {
         HH_CUDA(cudaMemsetAsync(d_bfill, 0, (size_t)nb * sizeof(unsigned int), ctx->stream));
         HH_CUDA(cudaMemsetAsync(d_agg, 0, 4 * sizeof(unsigned long long), ctx->stream));
         // ---- buckets: records per bucket, dense offsets, every record to its bucket
-        const int grid = hh_grid(ctx, 4);
+        int grid = 0, grid2 = 0;
+        HH_CHECK(hh_resident_grid(ctx, hh_k_part_hist, 512, 0, &grid));
+        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter2, 512, 0, &grid2));
         for (size_t k = 0; k < lk->psets.size(); ++k) {
             const hh_partset& ps = lk->psets[k];
             const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
@@ -1488,7 +1491,7 @@ static int links_finish_partitioned(hh_links* lk) {
         for (size_t k = 0; k < lk->psets.size(); ++k) {
             const hh_partset& ps = lk->psets[k];
             const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
-            HH_LAUNCH(ctx, hh_k_part_scatter2, grid, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
+            HH_LAUNCH(ctx, hh_k_part_scatter2, grid2, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
                       k == 0 ? (int64_t)n_spill : 0, blog, d_boff, d_bfill, d_rec2, compact_cap, lk->d_counters);
         }
         links_free_partsets(lk);                               // ordered on the stream behind scatter2
@@ -1498,10 +1501,9 @@ static int links_finish_partitioned(hh_links* lk) {
         // ---- every bucket in shared memory
         const size_t smem = (size_t)HH_AGG_SLOTS * (sizeof(uint64_t) + 7 * sizeof(uint32_t));
         HH_CUDA(cudaFuncSetAttribute(hh_k_bucket_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hh_k_bucket_count, HH_AGG_THREADS, smem));
-        HH_REQUIRE(per_sm > 0, HH_ERR_CUDA, "hh_links_finish: the bucket counting kernel does not fit an SM");
-        HH_LAUNCH(ctx, hh_k_bucket_count, hh_grid(ctx, per_sm), HH_AGG_THREADS, smem, d_rec2, d_boff, nb, hot, d_stage_compact,
+        int grid_agg = 0;
+        HH_CHECK(hh_resident_grid(ctx, hh_k_bucket_count, HH_AGG_THREADS, smem, &grid_agg));
+        HH_LAUNCH(ctx, hh_k_bucket_count, grid_agg, HH_AGG_THREADS, smem, d_rec2, d_boff, nb, hot, d_stage_compact,
                   compact_cap, lk->d_ctg, lk->d_counters, d_agg, d_fallback);
         unsigned long long agg[4];
         HH_CUDA(cudaMemcpyAsync(agg, d_agg, sizeof(agg), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1964,7 +1966,9 @@ extern "C" int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, i
             unsigned long long* d_out = reinterpret_cast<unsigned long long*>(ctx->d_scratch + 8);   // [0] touched  [1] passing
             HH_CUDA(cudaMemsetAsync(d_out, 0, 2 * sizeof(unsigned long long), ctx->stream));
             if (lk->nnz) {
-                const int grid = links_grid(ctx, lk->nnz);
+                int grid = 0;
+                HH_CHECK(hh_resident_grid(ctx, hh_k_touch, 256, 0, &grid));
+                grid = std::min(grid, links_grid(ctx, lk->nnz));
                 HH_LAUNCH(ctx, hh_k_touch, grid, 256, 0, lk->d_compact, lk->nnz, lk->d_keep, lk->d_ctg, normalize_by_nlinks,
                           hh_links_hap_dev(lk), w, d_touch, lk->d_deg, d_out + 1);
             }

@@ -148,10 +148,13 @@ extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, co
         if (sl) HH_LAUNCH(ctx, hh_k_mat_self_loops, (n + 255) / 256, 256, 0, n, m->d_colptr, m->d_row, m->d_val);
         int64_t nnz_c = 0;
         const uint32_t* compact = hh_links_compact(lk, &nnz_c);
-        const int gridc = (int)std::min<int64_t>((nnz_c + 255) / 256, (int64_t)ctx->sm_count * 8);
-        if (n_pass)
+        if (n_pass) {
+            int gridc = 0;
+            HH_CHECK(hh_resident_grid(ctx, hh_k_mat_scatter, 256, 0, &gridc));
+            gridc = (int)std::min<int64_t>((nnz_c + 255) / 256, gridc);
             HH_LAUNCH(ctx, hh_k_mat_scatter, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks, d_hap,
                       w, m->d_colptr, d_cursor, m->d_row, m->d_val);
+        }
         HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 10, d_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaStreamSynchronize(ctx->stream));
         const int err = *reinterpret_cast<int*>(ctx->h_scratch + 10);
