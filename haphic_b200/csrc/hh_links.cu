@@ -178,6 +178,9 @@ __device__ __forceinline__ bool hh_classify_contig(int4 r, int32_t n_ctg, const 
     return true;
 }
 
+// floor(x / d) for d > 0 (Python's //): bin number - 1 of the 0-based position x, ceil((x + 1) / d) - 1, for any x
+__device__ __forceinline__ int64_t hh_floor_div(int64_t x, int64_t d) { return x >= 0 ? x / d : -((-x + d - 1) / d); }
+
 // convert_frags (1662-1670) for one end on a split contig: the contig's first fragment f and the position p become the bin
 // and the position inside it.  false = the position names a bin that does not exist
 __device__ __forceinline__ bool hh_to_bin(int& f, int& p, int nbins, int64_t bin_size) {
@@ -203,7 +206,10 @@ __device__ __forceinline__ bool hh_classify_frag(int4 r, int32_t n_src, const in
     int fa = fbase[a], fb = fbase[b];
     const int na = fbase[a + 1] - fa, nb = fbase[b + 1] - fb;
     // a position outside the contig (.pairs position 0, or beyond the last bin) names a bin that does not exist: the
-    // reference dies with a KeyError on frag_len_dict['ctg_binK']; here the record is refused and hh_links_finish reports it
+    // reference dies with a KeyError on frag_len_dict['ctg_binK'] (1723); here the record is refused and hh_links_finish
+    // reports it.  Both ends of an intra-contig record in the same bin number -- existing or not -- are one fragment, which
+    // the reference skips (1715) before that lookup.
+    if (a == b && hh_floor_div((int64_t)pa, bin_size) == hh_floor_div((int64_t)pb, bin_size)) return false;
     bool bad = false;
     if (na > 1) bad = !hh_to_bin(fa, pa, na, bin_size);
     if (nb > 1) bad = !hh_to_bin(fb, pb, nb, bin_size) || bad;

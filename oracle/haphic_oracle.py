@@ -131,6 +131,131 @@ def count_links_c(pairs, lengths, name_rank, in_nx, flank_bp, cap=None):
             "ht": ht, "ctg_link_total": tot}
 
 
+# --------------------------------------------------------------------------------------
+# fragment mode: contigs longer than bin_size split into bins  (HapHiC_cluster.py:1658-1752, 188-296)
+# --------------------------------------------------------------------------------------
+
+def frag_records(pairs, frag_base, bin_size):
+    """parse_alignments' record handling (1696-1723) as a mapping of contig records into fragment space, after which
+    fragment-mode counting is contig-mode counting (count_links_* over fragment lengths / name ranks / Nx).
+
+    pairs: int [P, 4] (ctg_a, pos_a, ctg_b, pos_b), 0-based positions, ids of SOURCE contigs; frag_base [n_src + 1]:
+    contig c owns fragment ids [frag_base[c], frag_base[c+1]), more than one = split into bins of bin_size bp.
+    An end on a split contig at pos goes to bin k = ceil((pos + 1) / bin_size) (convert_frags, 1662-1670): fragment
+    frag_base[c] + k - 1 at position pos - (k - 1) * bin_size.  Rows are kept, so stream indices stay:
+      * ids outside [0, n_src) -> (-1, ., -1, .): skipped (1703);
+      * an intra-contig record whose ends share a bin number -> a == b: skipped (1699 / 1715), whether the bin exists or not;
+      * otherwise a bin outside 1..nbins -> (-1, ., -1, .) and REFUSED: the reference raises a KeyError (1723).
+    Returns (mapped int32 [P, 4], n_refused, stream indices of the refused records)."""
+    pairs = np.asarray(pairs).reshape(-1, 4)
+    step = 1 << 24                                     # int64 temporaries of 16 Mi records at a time
+    if len(pairs) > step:
+        out = np.empty((len(pairs), 4), np.int32)
+        bad = []
+        for lo in range(0, len(pairs), step):
+            out[lo:lo + step], _, b = frag_records(pairs[lo:lo + step], frag_base, bin_size)
+            bad.append(b + lo)
+        bad = np.concatenate(bad)
+        return out, len(bad), bad
+    p = pairs.astype(np.int64)
+    fb = np.asarray(frag_base, dtype=np.int64)
+    n_src = len(fb) - 1
+    a, pa, b, pb = p[:, 0], p[:, 1], p[:, 2], p[:, 3]
+    ok = (a >= 0) & (a < n_src) & (b >= 0) & (b < n_src)
+    a0, b0 = np.where(ok, a, 0), np.where(ok, b, 0)
+
+    def to_frag(c, pos):
+        nb = fb[c + 1] - fb[c]
+        k = -(-(pos + 1) // bin_size)                  # Python ceil: floor division, so any int32 position agrees
+        split = nb > 1
+        missing = split & ((k < 1) | (k > nb))
+        return np.where(split, fb[c] + k - 1, fb[c]), np.where(split, pos - (k - 1) * bin_size, pos), missing, k
+
+    fa, qa, miss_a, ka = to_frag(a0, pa)
+    fbb, qb, miss_b, kb = to_frag(b0, pb)
+    same_bin = ok & (a0 == b0) & (ka == kb)
+    refused = ok & (miss_a | miss_b) & ~same_bin
+    fa = np.where(same_bin, fb[a0], fa)
+    fbb = np.where(same_bin, fb[a0], fbb)
+    use = ok & ~refused
+    out = np.stack([np.where(use, fa, -1), np.where(use, qa, 0), np.where(use, fbb, -1), np.where(use, qb, 0)], 1)
+    bad = np.nonzero(refused)[0]
+    return out.astype(np.int32), len(bad), bad
+
+
+def count_frag_links_c(pairs, frag_base, bin_size, frag_len, frag_rank, frag_in_nx, flank_bp, cap=None):
+    """Every field of a fragment-mode table: count_links_c over frag_records.  Returns count_links_c's dict plus
+    "mapped", "n_refused" and "refused" (stream indices)."""
+    mapped, n_bad, bad = frag_records(pairs, frag_base, bin_size)
+    ref = count_links_c(mapped, frag_len, frag_rank, frag_in_nx, flank_bp, cap=cap)
+    ref.update(mapped=mapped, n_refused=n_bad, refused=bad)
+    return ref
+
+
+def count_frag_links_loop(pairs, names, lengths, bin_size, nx_frags, flank_bp):
+    """One Python iteration per record of parse_alignments (1696-1733) on name strings, with the reference's tuple sorts
+    and its fragment layout (stat_fragments, 228-264: contigs longer than bin_size split into '{ctg}_bin{k}').  For small
+    inputs; independent of frag_records.
+
+    pairs: int [P, 4] of contig ids into ``names`` (ids outside stand for names missing from the FASTA); nx_frags: the
+    set of Nx fragment names.  A record that would raise a KeyError in the reference (1723) is noted and skipped.
+    Returns a dict of insertion-ordered dicts keyed by names: "flank" {(frag_i, frag_j): n}, "frag_links" {frag: n},
+    "full" {(ctg_i, ctg_j): n} and "HT" {(ctg_i_H/T, ctg_j_H/T): n} (inter-contig records only, 1736-1746),
+    "ctg_pair_to_frag" {(ctg_i, ctg_j): {(frag_i, frag_j)}}, plus "frag_len" {frag: length} and "raises" (stream
+    indices of the records that would raise; the first is where the reference stops)."""
+    fa_dict = {n: int(ln) for n, ln in zip(names, np.asarray(lengths).tolist())}
+    split = {n for n, ln in fa_dict.items() if ln > bin_size}
+    frag_len = OrderedDict()
+    for n, ln in fa_dict.items():
+        if n in split:
+            nbins = -(-ln // bin_size)
+            for m in range(nbins):
+                frag_len["{}_bin{}".format(n, m + 1)] = bin_size if m + 1 < nbins else ln - m * bin_size
+        else:
+            frag_len[n] = ln
+
+    def convert(ctg, coord):                                   # 1662-1670
+        if ctg in split:
+            k = -(-coord // bin_size)
+            return "{}_bin{}".format(ctg, k), coord - (k - 1) * bin_size, True
+        return ctg, coord, False
+
+    full, flank_d, HT, frag_links, c2f = OrderedDict(), OrderedDict(), OrderedDict(), OrderedDict(), OrderedDict()
+    raises = []
+    n = len(names)
+    for r, (a, pa, b, pb) in enumerate(np.asarray(pairs).reshape(-1, 4).tolist()):
+        ref = names[a] if 0 <= a < n else None
+        mref = names[b] if 0 <= b < n else None
+        if ref == mref and ref not in split:                  # 1699
+            continue
+        if ref is None or mref is None:                        # 1703
+            continue
+        (ctg_i, coord_i), (ctg_j, coord_j) = sorted(((ref, pa + 1), (mref, pb + 1)))     # 1707
+        frag_i, fc_i, i_bin = convert(ctg_i, coord_i)
+        frag_j, fc_j, j_bin = convert(ctg_j, coord_j)
+        if frag_i == frag_j:                                   # 1715
+            continue
+        if i_bin or j_bin:                                     # 1719-1720
+            (frag_i, fc_i), (frag_j, fc_j) = sorted(((frag_i, fc_i), (frag_j, fc_j)))
+        if frag_i not in frag_len or frag_j not in frag_len:  # 1723: KeyError
+            raises.append(r)
+            continue
+        key = (frag_i, frag_j)
+        if frag_i in nx_frags and frag_j in nx_frags and is_flank(fc_i, frag_len[frag_i], flank_bp) and \
+                is_flank(fc_j, frag_len[frag_j], flank_bp):   # 1726-1729
+            flank_d[key] = flank_d.get(key, 0) + 1
+            frag_links[frag_i] = frag_links.get(frag_i, 0) + 1
+            frag_links[frag_j] = frag_links.get(frag_j, 0) + 1
+        c2f.setdefault((ctg_i, ctg_j), set()).add(key)         # 1732-1733
+        if ref != mref:                                        # 1736-1746
+            full[(ctg_i, ctg_j)] = full.get((ctg_i, ctg_j), 0) + 1
+            li, lj = fa_dict[ctg_i], fa_dict[ctg_j]
+            hk = (ctg_i + ("_T" if coord_i * 2 > li else "_H"), ctg_j + ("_T" if coord_j * 2 > lj else "_H"))
+            HT[hk] = HT.get(hk, 0) + 1
+    return {"flank": flank_d, "frag_links": frag_links, "full": full, "HT": HT, "ctg_pair_to_frag": c2f,
+            "frag_len": frag_len, "raises": raises}
+
+
 def count_links_numpy(pairs, lengths, name_rank, in_nx, flank_bp, with_clm=True):
     """Vectorised restatement of the same loop; identical outputs as arrays.
 

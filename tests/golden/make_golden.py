@@ -235,6 +235,96 @@ def link_case_bins(ref, tag, nchr, n_contigs, mean_len, n_pairs, flank, Nx, bin_
         tag, asm.n, len(frag_names), n_pairs, len(out["full_vals"]), len(out["flank_vals"])))
 
 
+def link_case_bins_edges(ref, tag, n_rec, flanks_kb, Nx, seed):
+    """Golden for parse_alignments at the edges of binning (tests/frag_edges.py): one stream counted with each flank
+    size, and the single records of frag_edges.SINGLE each parsed on its own with the outcome the reference gives it
+    (skipped, counted or a KeyError, which ends the reference's run)."""
+    import math
+    from tests import frag_edges as E
+    names = E.names()
+    rng = np.random.default_rng(seed)
+    pairs = E.stream(n_rec, seed + 1)
+    out = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        cwd = os.getcwd()
+        os.chdir(tmp)
+        try:
+            fasta = os.path.join(tmp, "asm.fa")
+            pfile = os.path.join(tmp, "aln.pairs")
+            with open(fasta, "w") as f:
+                for nm, ln in E.LAYOUT:
+                    f.write(">{}\n{}\n".format(nm, "".join(np.array(list("ACGT"))[rng.integers(0, 4, ln)])))
+            ext = names + [E.GHOST]
+
+            def write_pairs(path, rec):
+                with open(path, "w") as f:
+                    f.write("## pairs format v1.0\n")
+                    for r, (a, pa, b, pb) in enumerate(np.asarray(rec).tolist()):
+                        f.write("r{}\t{}\t{}\t{}\t{}\t+\t-\n".format(r, ext[a], pa + 1, ext[b], pb + 1))
+
+            write_pairs(pfile, pairs)
+            fa_dict = ref.parse_fasta(fasta, RE="GATC")
+            pos_t, dist_t = ref.determine_int_type(fa_dict)
+            _, bin_set, bin_size, frag_len_dict, Nx_frag_set, RE_site_dict, split_ctg_set = ref.stat_fragments(
+                fa_dict, "GATC", dict(), set(), nchrs=2, flank=flanks_kb[0], Nx=Nx, bin_size=E.BIN_KB)
+            frag_names, frag_base = [], [0]
+            for ctg, info in fa_dict.items():
+                if ctg in split_ctg_set:
+                    frag_names += ["{}_bin{}".format(ctg, k + 1) for k in range(math.ceil(info[1] / bin_size))]
+                else:
+                    frag_names.append(ctg)
+                frag_base.append(len(frag_names))
+            fid = {n: i for i, n in enumerate(frag_names)}
+            cid = {n: i for i, n in enumerate(names)}
+            out["names"] = np.array(names)
+            out["lengths"] = E.lengths()
+            out["pairs"] = pairs
+            out["ghost_id"] = np.int32(len(names))
+            out["Nx"] = np.int64(Nx)
+            out["bin_size"] = np.int64(bin_size)
+            out["flanks_kb"] = np.array(flanks_kb, np.int64)
+            out["frag_names"] = np.array(frag_names)
+            out["frag_base"] = np.array(frag_base, dtype=np.int32)
+            out["frag_len"] = np.array([frag_len_dict[f] for f in frag_names], dtype=np.int64)
+            out["frag_in_nx"] = np.array([f in Nx_frag_set for f in frag_names], dtype=np.uint8)
+            for fk in flanks_kb:
+                args = make_args(fasta=fasta, alignments=pfile, nchrs=2, flank=fk, Nx=Nx, bin_size=E.BIN_KB,
+                                 aln_format="pairs", remove_allelic_links=2)
+                full, flank_d, HT, _clm, frag_links, _coord, c2f = ref.parse_alignments(
+                    ref.pairs_generator(pfile, "pairs"), fa_dict, args, bin_size, frag_len_dict, Nx_frag_set, split_ctg_set,
+                    pos_t, dist_t)
+                p = "flank{}_".format(fk)
+                out[p + "keys"], out[p + "vals"] = dict_pairs_to_arrays(flank_d, fid, np.int64)
+                out[p + "frag_link_ids"] = np.array([fid[k] for k in frag_links.keys()], dtype=np.int32)
+                out[p + "frag_link_vals"] = np.array(list(frag_links.values()), dtype=np.int64)
+            # full / HT / ctg_pair_to_frag do not depend on the flank size
+            out["full_keys"], out["full_vals"] = dict_pairs_to_arrays(full, cid, np.int64)
+            hk = [(cid[a[:-2]], int(a.endswith("_T")), cid[b[:-2]], int(b.endswith("_T"))) for (a, b) in HT.keys()]
+            out["HT_keys"] = np.array(hk, dtype=np.int32).reshape(-1, 4)
+            out["HT_vals"] = np.array(list(HT.values()), dtype=np.int64)
+            out["c2f_json"] = np.array(json.dumps(sorted([[a, b, sorted(map(list, v))] for (a, b), v in c2f.items()])))
+            single, outcome = E.single_records(), []
+            for k in range(len(single)):
+                rec = single[k:k + 1]
+                sfile = os.path.join(tmp, "single{}.pairs".format(k))
+                write_pairs(sfile, rec)
+                try:
+                    _f, _fl, _h, _c, _t, _co, c2f1 = ref.parse_alignments(
+                        ref.pairs_generator(sfile, "pairs"), fa_dict, args, bin_size, frag_len_dict, Nx_frag_set,
+                        split_ctg_set, pos_t, dist_t)
+                    outcome.append(E.COUNTED if c2f1 else E.SKIPPED)
+                except KeyError:
+                    outcome.append(E.RAISES)
+            out["single_recs"] = single
+            out["single_outcome"] = np.array(outcome, np.int8)
+        finally:
+            os.chdir(cwd)
+    np.savez_compressed(os.path.join(HERE, "links_{}.npz".format(tag)), **out)
+    print("links_{}: n_ctg={} n_frag={} P={} nnz_full={} nnz_flank={} single outcomes={}".format(
+        tag, len(names), len(frag_names), n_rec, len(out["full_vals"]),
+        [len(out["flank{}_vals".format(fk)]) for fk in flanks_kb], out["single_outcome"].tolist()))
+
+
 def mcl_case(ref, tag, link_matrix, inflations, pruning=1e-4, expansion=2, max_iter=200, keep_iters=4):
     """Golden for MCL (a11-a15): first normalisation, pre-expansion, per-iteration matrices, clusters."""
     from sklearn.preprocessing import normalize
@@ -516,6 +606,8 @@ def main():
         link_case_bins(ref, "bins", nchr=3, n_contigs=45, mean_len=300000, n_pairs=60000, flank=40, Nx=90, bin_kb=100, seed=404)
         run_case(ref, "bins", nchr=3, n_contigs=60, mean_len=350000, n_pairs=120000, seed=505, Nx=100, bin_size=120, flank=60,
                  min_inflation=1.4, max_inflation=2.2, inflation_step=0.4)
+    if want("bins_edges"):
+        link_case_bins_edges(ref, "bins_edges", n_rec=6000, flanks_kb=(1, 5), Nx=70, seed=1212)
     if want("allelic"):
         allelic_case(ref, "p2", nchr=3, ploidy=2, n_contigs=120, mean_len=60000, n_pairs=120000, frac=0.2, seed=606, Nx=100)
         allelic_case(ref, "p4", nchr=2, ploidy=4, n_contigs=160, mean_len=50000, n_pairs=200000, frac=0.3, seed=707, Nx=100,
