@@ -66,6 +66,7 @@ _SIGNATURES = {
     "hh_ctx_device": (C.c_int, [_P]),
     "hh_ctx_sm_count": (C.c_int, [_P]),
     "hh_ctx_launches": (C.c_int64, [_P]),
+    "hh_ctx_mem_available": (C.c_int, [_P, C.POINTER(C.c_size_t)]),
     "hh_links_create": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int64, C.c_int64, C.POINTER(_P)]),
     "hh_links_create_frags": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, C.c_int64, C.c_int64, C.c_int64,
                                         C.POINTER(_P)]),
@@ -93,6 +94,8 @@ _SIGNATURES = {
     "hh_matrix_destroy": (C.c_int, [_P]),
     "hh_mcl_create": (C.c_int, [_P, C.c_int, C.c_int32, C.c_int32, C.POINTER(_P)]),
     "hh_mcl_create_ex": (C.c_int, [_P, C.c_int, C.c_int32, C.c_int32, C.c_int, C.POINTER(_P)]),
+    "hh_mcl_choose_preexp": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "hh_mcl_footprint": (C.c_int, [_P, C.c_int, C.c_int32, C.c_int, C.c_double, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "hh_mcl_preexp_info": (C.c_int, [_P, C.POINTER(PreexpInfo)]),
     "hh_mcl_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                               C.POINTER(C.c_float), C.POINTER(C.c_float)]),

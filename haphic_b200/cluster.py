@@ -824,7 +824,7 @@ def _mcl_sweep_multi_gpu(link_matrix, devices, expansion, inflations, max_iter, 
     import threading
     from ._lib import Context
     from .links import LinkMatrix
-    from .mcl import Mcl
+    from .mcl import Mcl, blocked_sweep
     host = link_matrix.to_scipy()                 # canonical (row-sorted) CSC: the same input on every device
     results = [None] * len(inflations)
     errors = []
@@ -833,11 +833,18 @@ def _mcl_sweep_multi_gpu(link_matrix, devices, expansion, inflations, max_iter, 
         try:
             ctx = _context() if dev == devices[0] else Context(dev)
             mat = LinkMatrix.from_csc(ctx, host)
-            engine = Mcl(mat, expansion, preexp=preexp)
-            for idx in range(k, len(inflations), len(devices)):
-                st = engine.run(float(inflations[idx]), max_iter, pruning)
-                results[idx] = (st, engine.result())
-            engine.close()
+            mine = list(range(k, len(inflations), len(devices)))
+            mode, blocks = _mcl_plan(mat, expansion, pruning, preexp)
+            if len(blocks) == 1:
+                engine = Mcl(mat, expansion, preexp=mode)
+                for idx in mine:
+                    st = engine.run(float(inflations[idx]), max_iter, pruning)
+                    results[idx] = (st, engine.result())
+                engine.close()
+            else:
+                sweep = blocked_sweep(mat, expansion, [inflations[idx] for idx in mine], max_iter, pruning, mode, blocks)
+                for idx, (_r, st, engine) in zip(mine, sweep):
+                    results[idx] = (st, engine.result())
             mat.close()
             if dev != devices[0]:
                 ctx.close()
@@ -856,12 +863,29 @@ def _mcl_sweep_multi_gpu(link_matrix, devices, expansion, inflations, max_iter, 
         yield inflation, mcl(None, expansion, float(inflation), max_iter, pruning, _done=done)
 
 
+def _mcl_budget(ctx):
+    """Device bytes one Markov-clustering engine may hold: what is available now, less a margin for the buffers a step
+    allocates for itself (packed blocks; the component-block GEMM of the early iterations, up to 8192 x n x 16 bytes, took
+    8.5 GB at 150k contigs)."""
+    from .mcl import available_bytes
+    return int(available_bytes(ctx) * 0.8)
+
+
+def _mcl_plan(link_matrix, expansion, pruning, preexp):
+    """(engine, column blocks) of the sweep: the whole pre-expanded matrix resident when it fits beside everything else the
+    engine holds, otherwise as few column blocks as fit (mcl.blocked_sweep).  The engine is resolved once for all blocks."""
+    from .mcl import footprint, plan_column_blocks, resolve_preexp
+    mode = resolve_preexp(link_matrix, expansion, preexp)
+    budget = _mcl_budget(link_matrix.ctx)
+    return mode, plan_column_blocks(link_matrix.n, lambda w: footprint(link_matrix, expansion, w, mode, pruning), budget)
+
+
 def run_mcl_clustering(link_matrix, bin_set, frag_len_dict, frag_index_dict, expansion, min_inflation,
                        max_inflation, inflation_step, max_iter, pruning, fa_dict, nchrs, dense_matrix):
     """run_mcl_clustering (2132-2242).  ``link_matrix`` is a device LinkMatrix (or anything scipy can
     turn into CSC, which is uploaded).  Writes inflation_*/ files, logs the recommendation."""
     from .links import LinkMatrix
-    from .mcl import Mcl, inflation_values
+    from .mcl import Mcl, blocked_sweep, inflation_values
     logger.info("Performing Markov clustering...")
     if not isinstance(link_matrix, LinkMatrix):
         link_matrix = LinkMatrix.from_csc(_context(), link_matrix)
@@ -876,9 +900,15 @@ def run_mcl_clustering(link_matrix, bin_set, frag_len_dict, frag_index_dict, exp
     if len(devices) > 1 and len(inflations) > 1:
         sweep = _mcl_sweep_multi_gpu(link_matrix, devices, expansion, inflations, max_iter, pruning, preexp)
     else:
-        engine = Mcl(link_matrix, expansion, preexp=preexp)
-        logger.debug("Pre-expansion engine: {} ({:.1f} ms)".format(engine.preexp["mode"], engine.preexp["total_ms"]))
-        sweep = ((inflation, mcl(engine, expansion, float(inflation), max_iter, pruning, dense_matrix)) for inflation in inflations)
+        mode, blocks = _mcl_plan(link_matrix, expansion, pruning, preexp)
+        logger.debug("Pre-expanded matrix: {} engine, {} column block(s) on the device at a time".format(mode, len(blocks)))
+        if len(blocks) == 1:
+            engine = Mcl(link_matrix, expansion, preexp=mode)
+            logger.debug("Pre-expansion engine: {} ({:.1f} ms)".format(engine.preexp["mode"], engine.preexp["total_ms"]))
+            sweep = ((inflation, mcl(engine, expansion, float(inflation), max_iter, pruning, dense_matrix)) for inflation in inflations)
+        else:
+            sweep = ((inflation, mcl(None, expansion, float(inflation), max_iter, pruning, _done=(st, eng.result())))
+                     for inflation, st, eng in blocked_sweep(link_matrix, expansion, inflations, max_iter, pruning, mode, blocks))
     result_clusters_list = []
     mcl_nrounds = 0
     for inflation, result in sweep:

@@ -177,6 +177,23 @@ bool hh_ws_release(hh_ctx* c, void* p) {
 
 void hh_ws_free_ptr(hh_ctx* c, void* p) { hh_ws_release(c, p); }
 
+// What the next large allocations can get: the small-allocation pool hands its unused memory back first (cudaMalloc of a
+// workspace block does not draw on it), and the idle workspace blocks count as free because a failed allocation releases them.
+extern "C" int hh_ctx_mem_available(hh_ctx* c, size_t* bytes) {
+    HH_REQUIRE(c && bytes, HH_ERR_ARG, "hh_ctx_mem_available: NULL argument");
+    HH_CUDA(cudaSetDevice(c->device));
+    HH_CUDA(cudaStreamSynchronize(c->stream));
+    cudaMemPool_t pool;
+    HH_CUDA(cudaDeviceGetDefaultMemPool(&pool, c->device));
+    HH_CUDA(cudaMemPoolTrimTo(pool, 0));
+    size_t free_b = 0, total_b = 0;
+    HH_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    for (size_t k = 0; k < c->ws->size(); ++k)
+        if (!(*c->ws)[k].used) free_b += (*c->ws)[k].bytes;
+    *bytes = free_b;
+    return HH_OK;
+}
+
 extern "C" int hh_ctx_sync(hh_ctx* c) {
     HH_REQUIRE(c != nullptr, HH_ERR_ARG, "hh_ctx_sync: ctx is NULL");
     HH_CUDA(cudaSetDevice(c->device));

@@ -468,12 +468,36 @@ int hh_gemm_passes(int na, int* pa, int* pb) {
     return np;
 }
 
+// The K range is cut into equal chunks when the operand planes of the whole range would exceed ~16 GB (a fifth of an 80 GB
+// device; 150k contigs: 135 GB): planes of one chunk at a time, the epilogue of every chunk after the first adds to M1.  The
+// cut depends on n and the encoding only, so every column block of M1 is cut alike and stays bit-identical.
+void hh_gemm_kchunks(int n, int planes, long long* kw_out, int* kchunks_out) {
+    const long long ldk = ((long long)n + 63) & ~63ll;
+    const double plane_bytes_all = (double)planes * (double)(ldk * (long long)n) * 2.0;
+    int kchunks = (int)(plane_bytes_all / 16.0e9) + 1;
+    kchunks = hg_env_int("HH_GEMM_KCHUNKS", kchunks);
+    if (kchunks < 1) kchunks = 1;
+    const long long kw = ((((long long)n + kchunks - 1) / kchunks) + 63) & ~63ll;      // chunk width, multiple of 64
+    *kw_out = kw;
+    *kchunks_out = (int)(((long long)n + kw - 1) / kw);
+}
+
+size_t hh_gemm_preexpand_plane_bytes(int n) {
+    size_t most = 0;
+    for (int planes : {3, 4, 6}) {            // scaled f16 (1 + 2), exact bf16 (1 + 3), weights (3 + 3)
+        long long kw = 0;
+        int kc = 0;
+        hh_gemm_kchunks(n, planes, &kw, &kc);
+        const size_t b = (size_t)planes * (size_t)kw * (size_t)n * 2;
+        if (b > most) most = b;
+    }
+    return most;
+}
+
 int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, float* d_m1, long long ld, const hh_gemm_item* h_items,
                       int n_items, hh_gemm_stats* st) {
     const int n = m->n;
     HH_REQUIRE(n >= 1 && n_items >= 1, HH_ERR_ARG, "hh_gemm_preexpand: empty problem");
-    const long long ldk = ((long long)n + 63) & ~63ll;       // row pitch in elements (128-byte multiple)
-    const long long plane = ldk * (long long)n;
     double* d_s = nullptr;
     float* d_inv = nullptr;
     int* d_flags = nullptr;
@@ -509,12 +533,9 @@ int hh_gemm_preexpand(hh_ctx* ctx, const hh_matrix* m, int col_lo, int col_hi, f
         // The K range is cut into equal chunks when the operand planes of the whole range would exceed ~16 GB (a fifth of an
         // 80 GB device; 150k contigs: 135 GB): planes of one chunk at a time, the epilogue of every chunk after the first adds to M1.  The cut depends on
         // n and the encoding only, so every rank of a sharded run cuts alike and M1 stays bit-identical for any world size.
-        const double plane_bytes_all = (double)(na + nb) * (double)plane * 2.0;
-        int kchunks = (int)(plane_bytes_all / 16.0e9) + 1;
-        kchunks = hg_env_int("HH_GEMM_KCHUNKS", kchunks);
-        if (kchunks < 1) kchunks = 1;
-        const long long kw = ((((long long)n + kchunks - 1) / kchunks) + 63) & ~63ll;      // chunk width, multiple of 64
-        kchunks = (int)(((long long)n + kw - 1) / kw);
+        long long kw = 0;
+        int kchunks = 0;
+        hh_gemm_kchunks(n, na + nb, &kw, &kchunks);
         const long long plane_c = kw * (long long)n;
         HH_CHECK(hh_ws_alloc(ctx, &d_A, (size_t)plane_c * (size_t)na));
         HH_CHECK(hh_ws_alloc(ctx, &d_B, (size_t)plane_c * (size_t)nb));

@@ -52,6 +52,11 @@ int hh_gemm_run(hh_ctx* ctx, const hh_gemm_operand& A, const hh_gemm_operand& B,
                 const int* pa, const int* pb, int chunk_kb, float* out, long long ld, int col_lo, int col_hi, const float* scale,
                 int* stages_out, float out_scale, int accumulate);
 int hh_gemm_passes(int na, int* pa, int* pb);
+// the K range cut of hh_gemm_preexpand for `planes` 16-bit operand planes of n x n: chunk width (multiple of 64), number of
+// chunks; the planes of one chunk take planes * kw * n * 2 bytes
+void hh_gemm_kchunks(int n, int planes, long long* kw, int* kchunks);
+// the largest operand planes of one K chunk hh_gemm_preexpand can allocate for n vertices, over every operand encoding
+size_t hh_gemm_preexpand_plane_bytes(int n);
 
 // operand planes of the block-diagonal iterate (row pitch ldk, rows = all n vertices): Bt from the slotted columns of `list`,
 // A by transposing inside every component.  f16 = 0: three exact bf16 planes each (six passes); f16 = 1: two f16 planes of

@@ -2331,6 +2331,52 @@ static int choose_preexp(const hh_matrix* m, int requested) {
     return (1.2 * t_dense < t_sparse) ? HH_PREEXP_DENSE : HH_PREEXP_SPARSE;
 }
 
+extern "C" int hh_mcl_choose_preexp(hh_matrix* m, int expansion, int requested, int* mode) {
+    HH_REQUIRE(m && mode, HH_ERR_ARG, "hh_mcl_choose_preexp: NULL argument");
+    hh_scope _scope(m->ctx);
+    HH_CUDA(cudaSetDevice(m->ctx->device));
+    *mode = (expansion == 2) ? choose_preexp(m, requested) : HH_PREEXP_SPARSE;
+    return HH_OK;
+}
+
+// slot entries of an iterate column: a column that sums to 1 holds at most 1/pruning entries >= pruning (+ slack for fp32
+// rounding)
+static int iterate_cap(int n, double pruning) {
+    if (pruning > 0.0 && 1.0 / pruning + 16.0 < (double)n) return (int)(1.0 / pruning) + 16;
+    return n;
+}
+
+static size_t slot_bytes(int n, int cap, int W) {
+    return (size_t)n * sizeof(int) + (size_t)n * (size_t)(W + 1) * sizeof(int) + (size_t)n * (size_t)cap * sizeof(uint2);
+}
+
+// mirrors the allocations of hh_mcl_create_ex and hh_mcl_begin (the transient buffers of a step below 32 MB are left out)
+extern "C" int hh_mcl_footprint(hh_matrix* m, int expansion, int32_t ncols, int mode, double pruning, size_t* m1_bytes,
+                                size_t* fixed_bytes) {
+    HH_REQUIRE(m && m1_bytes && fixed_bytes, HH_ERR_ARG, "hh_mcl_footprint: NULL argument");
+    HH_REQUIRE(mode == HH_PREEXP_SPARSE || mode == HH_PREEXP_DENSE, HH_ERR_ARG, "hh_mcl_footprint: mode must be SPARSE or DENSE");
+    HH_REQUIRE(0 < ncols && ncols <= m->n, HH_ERR_ARG, "hh_mcl_footprint: bad column count %d for n = %d", ncols, m->n);
+    hh_scope _scope(m->ctx);
+    hh_ctx* ctx = m->ctx;
+    HH_CUDA(cudaSetDevice(ctx->device));
+    const int n = m->n;
+    const hh_geom g = geom_for(ctx, n);
+    const int64_t ld = ((int64_t)n + 31) & ~31ll;
+    *m1_bytes = (size_t)ld * (size_t)ncols * sizeof(float);
+    size_t fixed = 0;
+    if (!g.smem_acc) fixed += (size_t)2 * (size_t)ctx->sm_count * (size_t)g.n_pad * sizeof(float);    // grid_cap_for: 2 per SM
+    fixed += (size_t)n * 11 * sizeof(int) + 64;          // order, 2n histogram, perm, inv, comp lo / hi, owned, lists, overflow
+    int cap0 = 0;
+    HH_CHECK(max_col_len(ctx, m, &cap0));
+    fixed += slot_bytes(n, cap0, g.W);
+    if (expansion > 2) fixed += slot_bytes(n, n, g.W) * (expansion > 3 ? 2 : 1);
+    if (expansion == 2 && mode == HH_PREEXP_DENSE)
+        fixed += hh_gemm_preexpand_plane_bytes(n) + (size_t)n * 24;     // + column sums, inverses, clip correction
+    fixed += 2 * slot_bytes(n, iterate_cap(n, pruning), g.W);
+    *fixed_bytes = fixed;
+    return HH_OK;
+}
+
 extern "C" int hh_mcl_create(hh_matrix* m, int expansion, int32_t col_lo, int32_t col_hi, hh_mcl** out) {
     return hh_mcl_create_ex(m, expansion, col_lo, col_hi, HH_PREEXP_AUTO, out);
 }
@@ -2720,9 +2766,7 @@ extern "C" int hh_mcl_begin(hh_mcl* mc, double inflation, double pruning) {
     hh_scope _scope(mc->ctx);
     HH_REQUIRE(inflation > 0.0, HH_ERR_ARG, "hh_mcl_begin: inflation must be positive");
     HH_CUDA(cudaSetDevice(mc->ctx->device));
-    // a column that sums to 1 holds at most 1/pruning entries >= pruning (+ slack for fp32 rounding)
-    int cap = mc->n;
-    if (pruning > 0.0 && 1.0 / pruning + 16.0 < (double)mc->n) cap = (int)(1.0 / pruning) + 16;
+    const int cap = iterate_cap(mc->n, pruning);
     if (cap != mc->it_cap) {
         slot_free(mc->it[0]);
         slot_free(mc->it[1]);

@@ -25,6 +25,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .mcl import continue_from_iteration0
+
 
 def column_blocks(n: int, world: int):
     """Contiguous, near-equal column blocks [(lo, hi)] * world."""
@@ -282,25 +284,11 @@ def sharded_mcl_sweep(engine, inflations, max_iter: int, pruning: float, blocks,
             saved[k] = None
             continue
         out, nnzs, prod0, ms0 = saved[k]
-        engine.begin(r, pruning)
-        engine.step(0)                                               # this rank's own block again (a 1/world stream of M1)
-        for rr in range(world):
-            if rr != rank:
-                c, z = ncols[rr], nnzs[rr]
-                engine.unpack(blocks[rr][0], blocks[rr][1], out[rr, :c], out[rr, c: c + z], out[rr, c + z: c + 2 * z].view(torch.float32))
-        engine.commit()
-        engine.set_block(0, n_total)
-        st = {"rounds": 1, "converged": False, "iter_nnz": [sum(nnzs)], "iter_products": [prod0], "iter_ms": [ms0], "owner": rank}
-        for it in range(1, max_iter):
-            nnz, prod, delta = engine.step(it)
-            engine.commit()
-            st["iter_nnz"].append(nnz)
-            st["iter_products"].append(prod)
-            st["iter_ms"].append(getattr(engine, "last_step_ms", 0.0))
-            st["rounds"] = it + 1
-            if it > 1 and delta <= 1e-8:
-                st["converged"] = True
-                break
+        # this rank's own block again (a 1/world stream of M1), then the others' from the saved buffers
+        others = ((blocks[rr][0], blocks[rr][1], out[rr, :ncols[rr]], out[rr, ncols[rr]: ncols[rr] + nnzs[rr]],
+                   out[rr, ncols[rr] + nnzs[rr]: ncols[rr] + 2 * nnzs[rr]].view(torch.float32)) for rr in range(world) if rr != rank)
+        st = continue_from_iteration0(engine, r, pruning, max_iter, n_total, others, (sum(nnzs), prod0, ms0))
+        st["owner"] = rank
         local[k] = st
         if on_result is not None:
             on_result(k, r, engine)

@@ -156,6 +156,163 @@ class Mcl:
             pass
 
 
+GEMM_TILE = 128       # column tile of the pre-expansion GEMM: block boundaries fall on its multiples
+
+
+def resolve_preexp(matrix: LinkMatrix, expansion: int, preexp: str = "auto") -> str:
+    """The pre-expansion engine hh_mcl_create_ex would pick now ("sparse" or "dense")."""
+    mode = C.c_int()
+    check(load().hh_mcl_choose_preexp(matrix._h, int(expansion), Mcl.PREEXP[preexp], C.byref(mode)))
+    return {HH_PREEXP_SPARSE: "sparse", HH_PREEXP_DENSE: "dense"}[mode.value]
+
+
+def footprint(matrix: LinkMatrix, expansion: int, ncols: int, mode: str, pruning: float = 1e-4):
+    """(M1 block bytes, bytes independent of ncols) an engine owning `ncols` columns holds on the device."""
+    m1, fixed = C.c_size_t(), C.c_size_t()
+    check(load().hh_mcl_footprint(matrix._h, int(expansion), int(ncols), Mcl.PREEXP[mode], float(pruning), C.byref(m1),
+                                  C.byref(fixed)))
+    return int(m1.value), int(fixed.value)
+
+
+def available_bytes(ctx) -> int:
+    """Device memory the next engine can allocate: free memory plus the library's idle cached blocks."""
+    b = C.c_size_t()
+    check(load().hh_ctx_mem_available(ctx.handle, C.byref(b)))
+    return int(b.value)
+
+
+def plan_column_blocks(n: int, footprint, budget: int, tile: int = GEMM_TILE):
+    """Contiguous column blocks [(lo, hi)] covering [0, n), as few as possible, each with sum(footprint(hi - lo)) <= budget.
+    Every boundary but n is a multiple of `tile`.  footprint(ncols) -> (M1 block bytes, fixed bytes), non-decreasing in ncols."""
+    def fits(w):
+        return sum(footprint(w)) <= budget
+
+    if fits(n):
+        return [(0, n)]
+    if not fits(min(tile, n)):
+        m1, fixed = footprint(min(tile, n))
+        raise MemoryError("Markov clustering needs {} bytes of device memory for one {}-column block of the pre-expanded "
+                          "matrix plus {} bytes that do not depend on the block; {} bytes are available".format(
+                              m1, min(tile, n), fixed, budget))
+
+    def widest(lo, hi, step):           # largest w in {lo, lo + step, ..., <= hi} that fits (lo fits)
+        a, b = lo // step, hi // step
+        while a < b:
+            mid = (a + b + 1) // 2
+            if fits(mid * step):
+                a = mid
+            else:
+                b = mid - 1
+        return a * step
+
+    w = widest(tile, n, tile)           # aligned blocks
+    last = widest(w, n, 1)              # the last block ends at n and need not be aligned
+    k = 1 + -(-(n - last) // w)
+    return [(i * w, (i + 1) * w) for i in range(k - 1)] + [((k - 1) * w, n)]
+
+
+def continue_from_iteration0(engine, inflation: float, pruning: float, max_iter: int, n: int, others, first):
+    """The rest of one mcl() call once iteration 0 of every column block exists: iteration 0 of the engine's own block
+    again, the other blocks unpacked (`others` yields (lo, hi, lengths, row indices, values) device tensors), and the
+    remaining iterations with every column owned -- the single-GPU code path.  `first` = (nnz, products, ms) of iteration 0
+    over all columns.  Returns {"rounds", "converged", "iter_nnz", "iter_products", "iter_ms", "iter_delta"}."""
+    engine.begin(inflation, pruning)
+    engine.step(0)
+    for lo, hi, ln, idx, val in others:
+        engine.unpack(lo, hi, ln, idx, val)
+    engine.commit()
+    engine.set_block(0, n)
+    st = {"rounds": 1, "converged": False, "iter_nnz": [first[0]], "iter_products": [first[1]], "iter_ms": [first[2]],
+          "iter_delta": [0.0]}
+    for it in range(1, max_iter):
+        nnz, prod, delta = engine.step(it)
+        engine.commit()
+        st["iter_nnz"].append(nnz)
+        st["iter_products"].append(prod)
+        st["iter_ms"].append(getattr(engine, "last_step_ms", 0.0))
+        st["iter_delta"].append(delta)
+        st["rounds"] = it + 1
+        if it > 1 and delta <= 1e-8:
+            st["converged"] = True
+            break
+    return st
+
+
+def _run_stats(st, n: int) -> dict:
+    """Statistics of continue_from_iteration0 in the form Mcl.run returns them (hh_mcl_run's byte count included)."""
+    nnz = np.asarray(st["iter_nnz"], np.int64)
+    moved = 4 * n * n + 8 * int(nnz[0]) + sum(16 * int(a) + 8 * int(b) + 12 * (n + 1) for a, b in zip(nnz[:-1], nnz[1:]))
+    return {"rounds": st["rounds"], "converged": st["converged"], "nnz": int(nnz[-1]), "products": int(sum(st["iter_products"])),
+            "bytes": moved, "iter_nnz": nnz, "iter_products": np.asarray(st["iter_products"], np.int64),
+            "iter_delta": np.asarray(st["iter_delta"], np.float32), "iter_ms": np.asarray(st["iter_ms"], np.float32)}
+
+
+def blocked_sweep(matrix: LinkMatrix, expansion: int, inflations, max_iter: int, pruning: float, mode: str, blocks,
+                  engine_cls=Mcl, timing: dict | None = None):
+    """An inflation sweep whose pre-expanded matrix M1 is never whole on the device.  Only iteration 0 of an mcl() call
+    reads M1, and its columns are independent, so:
+      phase A  one engine per column block in turn (M1 of that block only): iteration 0 of every inflation, the pruned
+               block kept in pinned host memory; every engine but the last is closed before the next one is built;
+      phase B  per inflation, the last block's engine rebuilds the whole iterate from the kept blocks and runs the
+               remaining iterations owning every column (continue_from_iteration0).
+    `mode` is the resolved engine ("sparse" / "dense"): every block must come from the same one.  Yields
+    (inflation, statistics as Mcl.run returns them, engine holding the result) in sweep order.  `timing` (optional) gets
+    the seconds of each phase and the device milliseconds of the pre-expansion over all blocks."""
+    import time
+
+    import torch
+    n = matrix.n
+    saved = [[] for _ in inflations]           # per inflation: (lo, hi, lengths, rows, values) of every block but the last
+    first = [[0, 0, 0.0] for _ in inflations]
+    engine = None
+    t0 = time.perf_counter()
+    try:
+        for b, (lo, hi) in enumerate(blocks):
+            if engine is not None:
+                engine.close()
+                engine = None
+                if torch.cuda.is_available():
+                    torch.cuda.empty_cache()   # the packed blocks went through torch's allocator: give the memory back
+            engine = engine_cls(matrix, expansion, lo, hi, preexp=mode)
+            if timing is not None:
+                timing["preexp_ms"] = timing.get("preexp_ms", 0.0) + getattr(engine, "preexp_ms", 0.0)
+            for k, r in enumerate(inflations):
+                engine.begin(float(r), pruning)
+                nnz, prod, _delta = engine.step(0)
+                first[k][0] += nnz
+                first[k][1] += prod
+                first[k][2] += getattr(engine, "last_step_ms", 0.0)
+                if b + 1 < len(blocks):
+                    host = []
+                    for t in engine.pack(nnz):
+                        h = torch.empty(t.shape, dtype=t.dtype, pin_memory=t.is_cuda)
+                        h.copy_(t)
+                        host.append(h)
+                    saved[k].append((lo, hi, *host))
+        if timing is not None:
+            timing["phase_a_s"] = time.perf_counter() - t0
+        dev = torch.device("cuda", engine.ctx.device) if getattr(engine, "ctx", None) is not None else torch.device("cpu")
+
+        def uploaded(k):
+            for lo, hi, ln, idx, val in saved[k]:
+                yield lo, hi, ln.to(dev), idx.to(dev), val.to(dev)
+            if dev.type == "cuda":
+                torch.cuda.empty_cache()      # the uploads are unpacked: leave their memory to the iterations
+
+        if timing is not None:
+            timing["phase_b_s"] = 0.0
+        for k, r in enumerate(inflations):
+            t1 = time.perf_counter()
+            st = continue_from_iteration0(engine, float(r), pruning, max_iter, n, uploaded(k), first[k])
+            saved[k] = None
+            if timing is not None:
+                timing["phase_b_s"] += time.perf_counter() - t1
+            yield r, _run_stats(st, n), engine
+    finally:
+        if engine is not None:
+            engine.close()
+
+
 def interpret_result(result):
     """Attractor rows -> clusters (HapHiC_cluster.py:2065-2095).  ``result`` is a scipy sparse
     matrix; returns a list of index tuples, or None when a node is in two clusters or in none."""

@@ -199,6 +199,16 @@ int hh_mcl_create(hh_matrix* m, int expansion, int32_t col_lo, int32_t col_hi, h
  * Both engines give M1 within fp32 rounding of the exact product; every later step is shared. */
 enum { HH_PREEXP_AUTO = 0, HH_PREEXP_SPARSE = 1, HH_PREEXP_DENSE = 2 };
 int hh_mcl_create_ex(hh_matrix* m, int expansion, int32_t col_lo, int32_t col_hi, int preexp_mode, hh_mcl** out);
+/* The engine hh_mcl_create_ex would pick for `requested` (SPARSE or DENSE; AUTO reads the free device memory now).  A sweep
+ * over column blocks resolves it once and passes the result to every block, so that all columns of M1 come from one engine. */
+int hh_mcl_choose_preexp(hh_matrix* m, int expansion, int requested, int* mode);
+/* Device bytes an engine created with hh_mcl_create_ex(m, expansion, lo, lo + ncols, mode) holds at its peak, for iterates
+ * pruned at `pruning`: m1_bytes = its dense block of M1 (grows with ncols), fixed_bytes = what does not depend on ncols
+ * (M0 slots, the global column accumulators above 57,600 vertices, the GEMM operand planes of one K chunk, the unpruned
+ * power slots of expansion > 2, the two iterate slots and the small per-vertex arrays).  mode must be SPARSE or DENSE. */
+int hh_mcl_footprint(hh_matrix* m, int expansion, int32_t ncols, int mode, double pruning, size_t* m1_bytes, size_t* fixed_bytes);
+/* free device memory plus the idle blocks of this context's workspace cache (released on demand by any allocation) */
+int hh_ctx_mem_available(hh_ctx* ctx, size_t* bytes);
 typedef struct {
     int32_t mode;          /* HH_PREEXP_SPARSE or HH_PREEXP_DENSE: what ran                              */
     int32_t a_planes;      /* dense: 16-bit planes of the count operand (1: integer counts, 3: weights)    */
