@@ -390,13 +390,56 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 #define HH_PART_TILE 4096          // records per tile of the scatter kernel (512 threads x 8)
 #define HH_PART_MAX 1024
 
-__global__ void __launch_bounds__(512)
+// The scatter kernels stage a tile's records in dynamic shared memory, ordered by destination (partition, or sub-bucket),
+// so that consecutive threads store the consecutive records of one run: a warp store then covers a few contiguous
+// stretches instead of 32 lines.  64 KiB per CTA beside 12 or 32 KiB of static arrays: two CTAs per SM, as the 62 / 63
+// registers x 512 threads allow anyway.
+#define HH_STAGE_SMEM ((size_t)HH_PART_TILE * sizeof(int4))
+
+// Exclusive prefix, in place, of the n <= 8 x 512 counts c[] of a tile, by its 512 threads; returns their sum.  s_wtot is
+// shared scratch of 16 words.  Barriers on entry (c[] is complete) and on exit (the prefix is visible).
+__device__ __forceinline__ unsigned int hh_tile_scan(unsigned int* c, int n, unsigned int* s_wtot) {
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const int per = (n + 511) >> 9, lo = threadIdx.x * per;
+    __syncthreads();
+    unsigned int sum = 0;
+    for (int k = 0; k < per; ++k)
+        if (lo + k < n) sum += c[lo + k];
+    unsigned int incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned int t = __shfl_up_sync(HH_FULL_MASK, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_wtot[wv] = incl;
+    __syncthreads();
+    unsigned int run = incl - sum, all = 0;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+        const unsigned int t = s_wtot[k];
+        run += (k < wv) ? t : 0u;
+        all += t;
+    }
+    for (int k = 0; k < per; ++k) {
+        if (lo + k < n) {
+            const unsigned int t = c[lo + k];
+            c[lo + k] = run;
+            run += t;
+        }
+    }
+    __syncthreads();
+    return all;
+}
+
+__global__ void __launch_bounds__(512, 2)
 hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_off, int32_t n_ctg, const int32_t* __restrict__ ctg_len,
                   const int32_t* __restrict__ name_rank, const uint8_t* __restrict__ in_nx, int64_t flank_bp, int npart_log,
                   int4* __restrict__ pbuf, uint64_t pcap, unsigned long long* __restrict__ cursor, int4* __restrict__ spill,
                   uint64_t spill_cap, unsigned long long* __restrict__ spill_cursor, unsigned long long* __restrict__ counters) {
-    __shared__ unsigned int s_cnt[HH_PART_MAX];
+    extern __shared__ int4 s_stage[];                // HH_PART_TILE records, ordered by partition
+    __shared__ unsigned int s_cnt[HH_PART_MAX];      // records of the tile per partition, then their exclusive prefix
     __shared__ unsigned long long s_base[HH_PART_MAX];
+    __shared__ unsigned int s_wtot[16];
     __shared__ unsigned int s_used;
     const int npart = 1 << npart_log;
     const int64_t tiles = (n_rec + HH_PART_TILE - 1) / HH_PART_TILE;
@@ -406,17 +449,15 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
         for (int k = threadIdx.x; k < npart; k += 512) s_cnt[k] = 0;
         __syncthreads();
         int4 out[8];
-        int part[8];
-        unsigned int rnk[8];
+        unsigned int rnk[8];                            // rank in the tile's run of its partition (.w >> 8), ~0 = none
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
             const int64_t i = t * HH_PART_TILE + (int64_t)k * 512 + threadIdx.x;
-            part[k] = -1;
+            rnk[k] = HH_NONE32;
             if (i < n_rec) {
                 hh_pair pr;
                 if (hh_classify_contig(hh_ld_stream(rec + i), n_ctg, ctg_len, name_rank, in_nx, flank_bp, &pr)) {
                     const int p = (int)(hh_mix64(hh_pair_key(pr.a, pr.b)) >> (64 - npart_log));
-                    part[k] = p;
                     rnk[k] = atomicAdd(&s_cnt[p], 1u);
                     out[k] = make_int4(pr.a, pr.b, (int)(stream_off + (uint32_t)i), (int)(pr.flags | ((unsigned)p << 8)));
                     my_used++;
@@ -426,17 +467,22 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
         __syncthreads();
         for (int k = threadIdx.x; k < npart; k += 512)
             if (s_cnt[k]) s_base[k] = atomicAdd(cursor + k, (unsigned long long)s_cnt[k]);
-        __syncthreads();
+        const unsigned int n_tile = hh_tile_scan(s_cnt, npart, s_wtot);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            if (part[k] < 0) continue;
-            const unsigned long long q = s_base[part[k]] + rnk[k];
+        for (int k = 0; k < 8; ++k)
+            if (rnk[k] != HH_NONE32) s_stage[s_cnt[(unsigned)out[k].w >> 8] + rnk[k]] = out[k];
+        __syncthreads();
+        // staged record e is number e - s_cnt[p] of the tile's run in partition p (p is in bits 8 and up of .w)
+        for (unsigned int e = threadIdx.x; e < n_tile; e += 512) {
+            const int4 r = s_stage[e];
+            const unsigned int p = (unsigned)r.w >> 8;
+            const unsigned long long q = s_base[p] + (e - s_cnt[p]);
             if (q < pcap) {
-                pbuf[(size_t)part[k] * (size_t)pcap + (size_t)q] = out[k];
+                pbuf[(size_t)p * (size_t)pcap + (size_t)q] = r;
             } else {
                 // the region of this partition is full (a few pairs own a large share of the stream): spill list
                 const unsigned long long sq = atomicAdd(spill_cursor, 1ull);
-                if (sq < spill_cap) spill[sq] = out[k];
+                if (sq < spill_cap) spill[sq] = r;
                 else atomicExch(counters + 2, 3ull);
             }
         }
@@ -497,13 +543,16 @@ hh_k_part_hist(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long
 }
 
 // The pass of hh_k_part_hist again: every record goes to boff[bucket] + its rank.  Ranks inside a tile come from shared
-// memory, one global atomic per (tile, sub-bucket) reserves the tile's run; bfill counts what each bucket received.
+// memory, one global atomic per (tile, sub-bucket) reserves the tile's run; bfill counts what each bucket received.  A
+// region tile is staged in shared memory ordered by sub-bucket and stored run by run.
 __global__ void __launch_bounds__(512, 2)
 hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int64_t tpr,
                    const int4* __restrict__ spill, int64_t n_spill, int bucket_log, const int64_t* __restrict__ boff,
                    unsigned int* __restrict__ bfill, int4* __restrict__ out, uint64_t n_out, unsigned long long* __restrict__ counters) {
-    __shared__ unsigned int s_cnt[1 << HH_SUB_MAX_LOG];
+    extern __shared__ int4 s_stage[];                    // HH_PART_TILE records, ordered by sub-bucket
+    __shared__ unsigned int s_cnt[1 << HH_SUB_MAX_LOG];  // records of the tile per sub-bucket, then their exclusive prefix
     __shared__ unsigned int s_base[1 << HH_SUB_MAX_LOG];
+    __shared__ unsigned int s_wtot[16];
     const int sub_log = bucket_log - npart_log, nsub = 1 << sub_log;
     const int64_t region_tiles = ((int64_t)1 << npart_log) * tpr;
     const int64_t tiles = region_tiles + (n_spill + HH_PART_TILE - 1) / HH_PART_TILE;
@@ -542,14 +591,18 @@ hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned 
         __syncthreads();
         for (int k = threadIdx.x; k < nsub; k += 512)
             if (s_cnt[k]) s_base[k] = atomicAdd(bfill + ((size_t)p << sub_log) + k, s_cnt[k]);
-        __syncthreads();
+        const unsigned int n_tile = hh_tile_scan(s_cnt, nsub, s_wtot);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            if (at[k] == HH_NONE32) continue;
-            const uint32_t sub = at[k] >> 16;
+        for (int k = 0; k < 8; ++k)
+            if (at[k] != HH_NONE32) s_stage[s_cnt[at[k] >> 16] + (at[k] & 0xFFFFu)] = r[k];
+        __syncthreads();
+        // staged record e is number e - s_cnt[sub] of the tile's run in its sub-bucket
+        for (unsigned int e = threadIdx.x; e < n_tile; e += 512) {
+            const int4 rec = s_stage[e];
+            const uint32_t sub = hh_bucket_of(rec, bucket_log) & (nsub - 1);
             const size_t b = ((size_t)p << sub_log) + sub;
-            const uint64_t q = (uint64_t)boff[b] + s_base[sub] + (at[k] & 0xFFFFu);
-            if (q < n_out) out[q] = r[k];
+            const uint64_t q = (uint64_t)boff[b] + s_base[sub] + (e - s_cnt[sub]);
+            if (q < n_out) out[q] = rec;
             else atomicExch(counters + 2, 6ull);
         }
         __syncthreads();
@@ -1305,10 +1358,11 @@ static int links_launch_insert(hh_links* lk, const int4* d_rec, int64_t n_rec, i
     if (lk->mode == 2 && d_pos == nullptr) {
         const int64_t tiles = (n_rec + HH_PART_TILE - 1) / HH_PART_TILE;
         int grid = 0;
-        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter, 512, 0, &grid));
+        HH_CUDA(cudaFuncSetAttribute(hh_k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HH_STAGE_SMEM));
+        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter, 512, HH_STAGE_SMEM, &grid));
         grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, grid));
         const hh_partset& ps = lk->psets.back();
-        HH_LAUNCH(ctx, hh_k_part_scatter, grid, 512, 0, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank, lk->d_nx,
+        HH_LAUNCH(ctx, hh_k_part_scatter, grid, 512, HH_STAGE_SMEM, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank, lk->d_nx,
                   lk->flank_bp, lk->npart_log, ps.buf, ps.pcap, ps.cursor, lk->d_spill, lk->spill_cap, lk->d_spill_cursor,
                   lk->d_counters);
         return HH_OK;
@@ -1486,7 +1540,8 @@ static int links_finish_partitioned(hh_links* lk) {
         // ---- buckets: records per bucket, dense offsets, every record to its bucket
         int grid = 0, grid2 = 0;
         HH_CHECK(hh_resident_grid(ctx, hh_k_part_hist, 512, 0, &grid));
-        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter2, 512, 0, &grid2));
+        HH_CUDA(cudaFuncSetAttribute(hh_k_part_scatter2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HH_STAGE_SMEM));
+        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter2, 512, HH_STAGE_SMEM, &grid2));
         for (size_t k = 0; k < lk->psets.size(); ++k) {
             const hh_partset& ps = lk->psets[k];
             const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
@@ -1497,7 +1552,7 @@ static int links_finish_partitioned(hh_links* lk) {
         for (size_t k = 0; k < lk->psets.size(); ++k) {
             const hh_partset& ps = lk->psets[k];
             const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
-            HH_LAUNCH(ctx, hh_k_part_scatter2, grid2, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
+            HH_LAUNCH(ctx, hh_k_part_scatter2, grid2, 512, HH_STAGE_SMEM, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
                       k == 0 ? (int64_t)n_spill : 0, blog, d_boff, d_bfill, d_rec2, compact_cap, lk->d_counters);
         }
         links_free_partsets(lk);                               // ordered on the stream behind scatter2
