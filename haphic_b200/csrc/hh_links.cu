@@ -377,14 +377,15 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 // read-modify-write for the counters (the table is two orders of magnitude larger than L2).  For long streams the
 // records are therefore split twice by the high bits of the key hash: into 2^npart_log partition regions while they
 // stream in, and at finish into 2^bucket_log buckets (the next hash bits, links_bucket_log) laid out densely.  A bucket
-// (about 1.3k records at the benchmark's 200M records) is then counted in an open-addressing table in shared memory and emitted as
-// compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only: the result is identical to
+// (about 1.3k records at the benchmark's 200M records) is then sorted by pair in shared memory, its runs are reduced, and
+// it is emitted as compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only: the result is identical to
 // the direct path.
 //   hh_k_part_scatter   record -> {i, j, stream index, flags} (ends ordered by name rank, is_flank / head-tail evaluated once)
 //   hh_k_part_hist      records per bucket (shared-memory histogram of a region's sub-buckets per tile)
 //   hh_k_part_scatter2  the same pass again: every record to its place in the dense bucket buffer
-//   hh_k_bucket_count   persistent CTAs: count one bucket at a time in shared memory, emit its live slots, clear
-//   hh_k_part_step      fallback for the buckets a shared-memory table cannot take: gathered, then counted in batches of
+//   hh_k_bucket_count   persistent CTAs: count one bucket at a time in shared memory (sort by pair, reduce the runs),
+//                       emit its entries
+//   hh_k_part_step      fallback for the buckets shared memory does not take: gathered, then counted in batches of
 //                       about 2^19 records through global scratch tables
 // ---------------------------------------------------------------------------------------------
 #define HH_PART_TILE 4096          // records per tile of the scatter kernel (512 threads x 8)
@@ -498,7 +499,8 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 // A bucket is the top bucket_log bits of hh_mix64(key): the partition (top npart_log bits) and below it a sub-bucket.
 #define HH_AGG_MEAN 2048           // buckets hold at most this many records on average (links_bucket_log)
 #define HH_SUB_MAX_LOG 12          // at most 2^12 sub-buckets per partition region: the shared histograms of hist / scatter2
-#define HH_AGG_SLOTS 2048          // slots of a shared-memory table (36 B each: 72 KiB, three CTAs per SM)
+#define HH_AGG_SLOTS 2048          // the largest table of the fallback rule (tsize in hh_k_bucket_count)
+#define HH_AGG_LIST (HH_AGG_SLOTS / 4 * 3)   // the largest distinct-pair limit: entries of a bucket's aggregate list
 #define HH_AGG_THREADS 256
 #define HH_AGG_HOT 32              // a bucket with more than HH_AGG_HOT x the mean records skips shared memory (links_hot_records)
 
@@ -609,139 +611,252 @@ hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned 
     }
 }
 
-// Count every bucket in shared memory.  Persistent CTAs take buckets from an atomic queue (agg[0]).  A bucket's table is
-// the power of two >= 1.5 x its records (at least one slot per thread, at most HH_AGG_SLOTS), stored SoA: u64 keys and
-// the seven u32 counters of hh_slot.  Nothing leaves the CTA before the bucket has counted completely: a bucket whose
-// distinct keys exceed 3/4 of the table (or whose probe finds no slot) is abandoned -- its table is cleared and it goes
-// on the fallback list (agg[1] entries), as does a bucket of more than `hot` records.  A completed bucket is emitted
-// (one global atomic reserves its entries, a block scan per 256 slots ranks them, so a warp writes consecutive entries),
-// with the per-fragment totals and nnz_flank, and only the slots it used are cleared.  agg[2] counts completed buckets.
+// Count every bucket in shared memory.  Persistent CTAs take buckets from an atomic queue (agg[0]) and read a bucket in
+// chunks of S = 256 x ITEMS records.  A chunk is sorted by its exact pair key (i << kbits) | j (block radix sort over the
+// 2 kbits key bits; payload: the record's place in the chunk and its flags), the runs of equal keys are reduced by one
+// segmented block scan, and the runs are merged into the bucket's aggregate list, a key-sorted SoA list in shared memory
+// of at most HH_AGG_LIST entries: a run whose key is on the list adds to its entry, the new ones are placed by their rank
+// among the new keys plus their lower bound on the list (merge path).  The fallback rule: with tsize the power of two
+// >= 1.5 x the bucket's records (256 .. HH_AGG_SLOTS), a bucket with more than tsize / 4 x 3 distinct pairs (checked
+// after every chunk; the count only grows) goes on the fallback list (agg[1] entries), as does a bucket of more than `hot`
+// records.  Nothing leaves the CTA before the bucket has counted completely.  A completed bucket reserves its entries with
+// one global atomic and writes them word by word (consecutive threads, consecutive words), with the per-fragment totals
+// and nnz_flank.  agg[2] counts completed buckets.
+#define HH_PK_FLANK 12             // a run's counters packed 12 bits each (a chunk has at most 2048 < 2^12 records)
+#define HH_PK_HT 24
+#define HH_PK_TH 36
+#define HH_PK_TT 48
+#define HH_PK_MASK 0xFFFull
+#define HH_PK_HEAD (1ull << 63)    // a run starts at this record
+
+struct hh_run {
+    unsigned long long c;            // full | flank << 12 | HT << 24 | TH << 36 | TT << 48 | head << 63
+    uint32_t first_full, first_flank;
+};
+
+// segmented sum / min: a head on the right starts over
+struct hh_run_op {
+    __device__ __forceinline__ hh_run operator()(const hh_run& a, const hh_run& b) const {
+        if (b.c & HH_PK_HEAD) return b;
+        return hh_run{a.c + b.c, min(a.first_full, b.first_full), min(a.first_flank, b.first_flank)};
+    }
+};
+
+template <typename K>
+__device__ __forceinline__ int hh_lower_bound(const K* a, int n, K k) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a[mid] < k) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// 32-bit keys up to 65,536 objects: chunks of 2048 records; 64-bit keys: 1280.  Three CTAs per SM (80 registers).
+template <typename K, int ITEMS>
+struct hh_bc_smem {
+    typedef cub::BlockRadixSort<K, HH_AGG_THREADS, ITEMS, uint32_t> sort_t;
+    typedef cub::BlockScan<hh_run, HH_AGG_THREADS> run_scan_t;
+    typedef cub::BlockScan<unsigned int, HH_AGG_THREADS> cnt_scan_t;
+    K key[HH_AGG_LIST];                              // the aggregate list, ascending keys
+    uint32_t val[HH_E_WORDS - 2][HH_AGG_LIST];       // its counters, word w of an entry in val[w - 2]
+    uint32_t z[HH_AGG_THREADS * ITEMS];              // stream index of the chunk's records
+    union {
+        typename sort_t::TempStorage sort;
+        struct {
+            K first[HH_AGG_THREADS], last[HH_AGG_THREADS];   // every thread's first / last key after the sort
+        } edge;
+        K fresh[HH_AGG_THREADS * ITEMS];             // the chunk's keys that are not on the list, ascending
+    } u;
+    typename run_scan_t::TempStorage run_scan;
+    typename cnt_scan_t::TempStorage cnt_scan;
+    unsigned long long base;
+    int bucket;
+};
+
+template <typename K, int ITEMS>
 __global__ void __launch_bounds__(HH_AGG_THREADS, 3)
-hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff, int nbuckets, uint64_t hot,
+hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff, int nbuckets, uint64_t hot, int kbits,
                   uint32_t* __restrict__ compact, uint64_t compact_cap, unsigned long long* __restrict__ ctg_links,
                   unsigned long long* __restrict__ counters, unsigned long long* __restrict__ agg, uint32_t* __restrict__ fallback) {
+    typedef hh_bc_smem<K, ITEMS> smem_t;
+    constexpr int S = HH_AGG_THREADS * ITEMS;
     extern __shared__ __align__(16) unsigned char hh_agg_smem[];
-    uint64_t* tkey = reinterpret_cast<uint64_t*>(hh_agg_smem);
-    uint32_t* t_full = reinterpret_cast<uint32_t*>(tkey + HH_AGG_SLOTS);
-    uint32_t* t_flank = t_full + HH_AGG_SLOTS;
-    uint32_t* t_ffull = t_flank + HH_AGG_SLOTS;
-    uint32_t* t_fflank = t_ffull + HH_AGG_SLOTS;
-    uint32_t* t_ht = t_fflank + HH_AGG_SLOTS;
-    uint32_t* t_th = t_ht + HH_AGG_SLOTS;
-    uint32_t* t_tt = t_th + HH_AGG_SLOTS;
-    __shared__ int s_bucket;
-    __shared__ unsigned int s_distinct, s_abandon;
-    __shared__ unsigned int s_wtot[HH_AGG_THREADS / 32];
-    __shared__ unsigned long long s_base;
-    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
-    auto clear = [&](int s) {
-        tkey[s] = HH_EMPTY_KEY;
-        t_full[s] = 0u;
-        t_flank[s] = 0u;
-        t_ffull[s] = HH_NONE32;
-        t_fflank[s] = HH_NONE32;
-        t_ht[s] = 0u;
-        t_th[s] = 0u;
-        t_tt[s] = 0u;
-    };
-    for (int s = threadIdx.x; s < HH_AGG_SLOTS; s += HH_AGG_THREADS) clear(s);
+    smem_t& sm = *reinterpret_cast<smem_t*>(hh_agg_smem);
+    const int t = threadIdx.x;
+    const K jmask = ((K)1 << kbits) - 1;
+    const hh_run none = {HH_PK_HEAD, HH_NONE32, HH_NONE32};
     unsigned int nfl = 0, n_done = 0;
     for (;;) {
         __syncthreads();                            // the previous bucket is finished with every shared variable
-        if (threadIdx.x == 0) {
-            s_bucket = (int)atomicAdd(agg + 0, 1ull);
-            s_distinct = 0;
-            s_abandon = 0;
-        }
+        if (t == 0) sm.bucket = (int)atomicAdd(agg + 0, 1ull);
         __syncthreads();
-        const int bk = s_bucket;
+        const int bk = sm.bucket;
         if (bk >= nbuckets) break;
         const int64_t lo = boff[bk], n = boff[bk + 1] - lo;
         if ((uint64_t)n > hot) {
-            if (threadIdx.x == 0) fallback[atomicAdd(agg + 1, 1ull)] = (uint32_t)bk;
+            if (t == 0) fallback[atomicAdd(agg + 1, 1ull)] = (uint32_t)bk;
             continue;
         }
         int tsize = HH_AGG_THREADS;
         while (tsize < HH_AGG_SLOTS && (int64_t)tsize * 2 < n * 3) tsize <<= 1;
-        const unsigned int limit = (unsigned)tsize / 4 * 3;
-        const unsigned int mask = (unsigned)tsize - 1;
-        // ---- count
-        for (int64_t i0 = (int64_t)wv * 32; i0 < n; i0 += HH_AGG_THREADS) {
-            const int64_t i = i0 + lane;
-            const bool ok = i < n;
-            int4 r = make_int4(0, 0, 0, 0);
-            if (ok) r = hh_ld_stream(rec + lo + i);
-            const uint64_t key = hh_pair_key(r.x, r.y);
-            const hh_group g = hh_warp_fold(ok, key, (uint32_t)r.z, (unsigned)r.w);
-            if (g.leader) {
-                unsigned int slot = (unsigned int)hh_mix64(key) & mask;
-                int probes = 0;
-                for (; probes < tsize; ++probes) {
-                    const uint64_t k = *((volatile uint64_t*)(tkey + slot));
-                    if (k == key) break;
-                    if (k == HH_EMPTY_KEY) {
-                        const unsigned long long prev = atomicCAS((unsigned long long*)(tkey + slot), (unsigned long long)HH_EMPTY_KEY,
-                                                                  (unsigned long long)key);
-                        if (prev == HH_EMPTY_KEY) {
-                            if (atomicAdd(&s_distinct, 1u) >= limit) s_abandon = 1;
-                            break;
-                        }
-                        if (prev == key) break;
-                    }
-                    slot = (slot + 1) & mask;
-                }
-                if (probes == tsize) {
-                    s_abandon = 1;
-                } else {
-                    atomicAdd(t_full + slot, g.full);
-                    atomicMin(t_ffull + slot, g.first_all);
-                    if (g.flank) {
-                        atomicAdd(t_flank + slot, g.flank);
-                        atomicMin(t_fflank + slot, g.first_flank);
-                    }
-                    if (g.ht) atomicAdd(t_ht + slot, g.ht);
-                    if (g.th) atomicAdd(t_th + slot, g.th);
-                    if (g.tt) atomicAdd(t_tt + slot, g.tt);
+        const int limit = tsize / 4 * 3;
+        int na = 0;                                 // entries on the aggregate list (block-uniform)
+        bool abandon = false;
+        for (int64_t c0 = 0; c0 < n; c0 += S) {
+            const int m = (int)min((int64_t)S, n - c0);
+            // ---- load (striped: a warp reads consecutive records) and sort.  Padding sorts last: a real key has i != j,
+            // so its 2 kbits are never all ones.
+            K key[ITEMS];
+            uint32_t pay[ITEMS];                    // place in the chunk | flags << 11 | (merge: 1 + lower bound of a new run) << 16
+            __syncthreads();                        // the previous chunk is finished with z and the list
+#pragma unroll
+            for (int q = 0; q < ITEMS; ++q) {
+                const int l = q * HH_AGG_THREADS + t;
+                key[q] = ~(K)0;
+                pay[q] = 0;
+                if (l < m) {
+                    const int4 r = hh_ld_stream(rec + lo + c0 + l);
+                    key[q] = ((K)(uint32_t)r.x << kbits) | (K)(uint32_t)r.y;
+                    pay[q] = (uint32_t)l | (((uint32_t)r.w & 7u) << 11);
+                    sm.z[l] = (uint32_t)r.z;
                 }
             }
-            if (__any_sync(HH_FULL_MASK, *((volatile unsigned int*)&s_abandon) != 0)) break;
+            typename smem_t::sort_t(sm.u.sort).Sort(key, pay, 0, 2 * kbits);
+            // ---- reduce: thread t holds sorted places t * ITEMS + q
+            __syncthreads();
+            sm.u.edge.first[t] = key[0];
+            sm.u.edge.last[t] = key[ITEMS - 1];
+            __syncthreads();
+            const K prev = t > 0 ? sm.u.edge.last[t - 1] : ~(K)0;
+            const K next = t + 1 < HH_AGG_THREADS ? sm.u.edge.first[t + 1] : ~(K)0;
+            auto item = [&](int q) -> hh_run {
+                const int pos = t * ITEMS + q;
+                if (pos >= m) return none;
+                const unsigned f = (pay[q] >> 11) & 7u;
+                const uint32_t z = sm.z[pay[q] & 0x7FFu];
+                const bool fl = f & HH_F_FLANK, ti = f & HH_F_TI, tj = f & HH_F_TJ;
+                hh_run r;
+                const bool head = pos == 0 || key[q] != (q ? key[q - 1] : prev);
+                r.c = 1ull | ((unsigned long long)head << 63) | ((unsigned long long)fl << HH_PK_FLANK) | ((unsigned long long)(!ti && tj) << HH_PK_HT) |
+                      ((unsigned long long)(ti && !tj) << HH_PK_TH) | ((unsigned long long)(ti && tj) << HH_PK_TT);
+                r.first_full = z;
+                r.first_flank = fl ? z : HH_NONE32;
+                return r;
+            };
+            const hh_run_op op;
+            hh_run acc = item(0);
+#pragma unroll
+            for (int q = 1; q < ITEMS; ++q) acc = op(acc, item(q));
+            hh_run carry;                           // the open run of the threads before this one
+            typename smem_t::run_scan_t(sm.run_scan).ExclusiveScan(acc, carry, hh_run{0ull, HH_NONE32, HH_NONE32}, op);
+            // ---- merge, step 1: runs whose key is on the list add to its entry; the others are new
+            unsigned int nnew = 0;
+            hh_run run = carry;
+#pragma unroll
+            for (int q = 0; q < ITEMS; ++q) {
+                run = op(run, item(q));
+                const int pos = t * ITEMS + q;
+                if (pos < m && (pos + 1 == m || key[q] != (q + 1 < ITEMS ? key[q + 1] : next))) {
+                    const int lb = hh_lower_bound(sm.key, na, key[q]);
+                    if (lb < na && sm.key[lb] == key[q]) {
+                        sm.val[HH_E_FULL - 2][lb] += (uint32_t)(run.c & HH_PK_MASK);
+                        sm.val[HH_E_FLANK - 2][lb] += (uint32_t)((run.c >> HH_PK_FLANK) & HH_PK_MASK);
+                        sm.val[HH_E_FIRST_FULL - 2][lb] = min(sm.val[HH_E_FIRST_FULL - 2][lb], run.first_full);
+                        sm.val[HH_E_FIRST_FLANK - 2][lb] = min(sm.val[HH_E_FIRST_FLANK - 2][lb], run.first_flank);
+                        sm.val[HH_E_HT - 2][lb] += (uint32_t)((run.c >> HH_PK_HT) & HH_PK_MASK);
+                        sm.val[HH_E_TH - 2][lb] += (uint32_t)((run.c >> HH_PK_TH) & HH_PK_MASK);
+                        sm.val[HH_E_TT - 2][lb] += (uint32_t)((run.c >> HH_PK_TT) & HH_PK_MASK);
+                    } else {
+                        pay[q] |= (uint32_t)(lb + 1) << 16;
+                        nnew++;
+                    }
+                }
+            }
+            unsigned int rank, fresh;
+            typename smem_t::cnt_scan_t(sm.cnt_scan).ExclusiveSum(nnew, rank, fresh);
+            if (na + (int)fresh > limit) {
+                abandon = true;
+                break;
+            }
+            if (fresh == 0) continue;
+            // ---- merge, step 2: an entry of the list moves up by the new keys below it.  Destinations are >= sources, so
+            // groups of 256 entries move from the top down, each read completely before it is written.
+            if (na) {
+                unsigned int r = rank;
+#pragma unroll
+                for (int q = 0; q < ITEMS; ++q)
+                    if (pay[q] >> 16) sm.u.fresh[r++] = key[q];
+                __syncthreads();
+                for (int hi = na; hi > 0; hi -= HH_AGG_THREADS) {
+                    const int a = hi - HH_AGG_THREADS + t;
+                    K k = 0;
+                    uint32_t v[HH_E_WORDS - 2];
+                    int d = a;                      // stays: no entry, or one that does not move
+                    if (a >= 0) {
+                        k = sm.key[a];
+#pragma unroll
+                        for (int w = 0; w < HH_E_WORDS - 2; ++w) v[w] = sm.val[w][a];
+                        d = a + hh_lower_bound(sm.u.fresh, (int)fresh, k);
+                    }
+                    __syncthreads();
+                    if (d > a) {
+                        sm.key[d] = k;
+#pragma unroll
+                        for (int w = 0; w < HH_E_WORDS - 2; ++w) sm.val[w][d] = v[w];
+                    }
+                    __syncthreads();
+                }
+            }
+            // ---- merge, step 3: the new runs, reduced again (fewer registers than keeping them), take the places left free
+            run = carry;
+#pragma unroll
+            for (int q = 0; q < ITEMS; ++q) {
+                run = op(run, item(q));
+                if ((pay[q] >> 16) == 0) continue;
+                const int d = (int)(pay[q] >> 16) - 1 + (int)rank++;
+                const hh_run& o = run;
+                sm.key[d] = key[q];
+                sm.val[HH_E_FULL - 2][d] = (uint32_t)(o.c & HH_PK_MASK);
+                sm.val[HH_E_FLANK - 2][d] = (uint32_t)((o.c >> HH_PK_FLANK) & HH_PK_MASK);
+                sm.val[HH_E_FIRST_FULL - 2][d] = o.first_full;
+                sm.val[HH_E_FIRST_FLANK - 2][d] = o.first_flank;
+                sm.val[HH_E_HT - 2][d] = (uint32_t)((o.c >> HH_PK_HT) & HH_PK_MASK);
+                sm.val[HH_E_TH - 2][d] = (uint32_t)((o.c >> HH_PK_TH) & HH_PK_MASK);
+                sm.val[HH_E_TT - 2][d] = (uint32_t)((o.c >> HH_PK_TT) & HH_PK_MASK);
+            }
+            na += (int)fresh;
         }
-        __syncthreads();
-        if (s_abandon) {
-            for (int s = threadIdx.x; s < tsize; s += HH_AGG_THREADS) clear(s);
-            if (threadIdx.x == 0) fallback[atomicAdd(agg + 1, 1ull)] = (uint32_t)bk;
+        if (abandon) {
+            if (t == 0) fallback[atomicAdd(agg + 1, 1ull)] = (uint32_t)bk;
             continue;
         }
-        // ---- emit + clear
-        if (threadIdx.x == 0) s_base = s_distinct ? atomicAdd(counters + 0, (unsigned long long)s_distinct) : 0ull;
+        // ---- emit: entry e of the list is entry base + e, word w of it is compact word base x 9 + w
         __syncthreads();
-        unsigned long long run = s_base;
-        for (int s0 = 0; s0 < tsize; s0 += HH_AGG_THREADS) {
-            const int s = s0 + threadIdx.x;
-            const uint64_t key = tkey[s];
-            const bool live = key != HH_EMPTY_KEY;
-            unsigned int total;
-            const unsigned long long pos = run + hh_block_rank(live ? 1u : 0u, s_wtot, &total);
-            if (live) {
-                const uint32_t flank = t_flank[s];
-                if (pos < compact_cap)
-                    hh_entry_store(compact + pos * HH_E_WORDS, key, t_full[s], flank, t_ffull[s], t_fflank[s], t_ht[s], t_th[s], t_tt[s]);
-                else
-                    atomicExch(counters + 2, 5ull);
-                if (flank) {
-                    nfl++;
-                    atomicAdd(ctg_links + (uint32_t)(key >> 32), (unsigned long long)flank);      // ctg_link_dict (1638-1639)
-                    atomicAdd(ctg_links + (uint32_t)key, (unsigned long long)flank);
-                }
-                clear(s);
+        if (t == 0) sm.base = na ? atomicAdd(counters + 0, (unsigned long long)na) : 0ull;
+        __syncthreads();
+        const unsigned long long base = sm.base;
+        for (int w = t; w < na * HH_E_WORDS; w += HH_AGG_THREADS) {
+            const int e = w / HH_E_WORDS, f = w - e * HH_E_WORDS;
+            const uint32_t x = f == HH_E_I ? (uint32_t)(sm.key[e] >> kbits)
+                             : f == HH_E_J ? (uint32_t)(sm.key[e] & jmask) : sm.val[f - 2][e];
+            if (base + e < compact_cap) compact[base * HH_E_WORDS + w] = x;
+            else atomicExch(counters + 2, 5ull);
+        }
+        for (int e = t; e < na; e += HH_AGG_THREADS) {
+            const uint32_t flank = sm.val[HH_E_FLANK - 2][e];
+            if (flank) {
+                nfl++;
+                atomicAdd(ctg_links + (uint32_t)(sm.key[e] >> kbits), (unsigned long long)flank);    // ctg_link_dict (1638-1639)
+                atomicAdd(ctg_links + (uint32_t)(sm.key[e] & jmask), (unsigned long long)flank);
             }
-            run += total;
         }
         n_done++;
     }
     nfl = (unsigned)hh_warp_sum((int)nfl);
-    if (lane == 0 && nfl) atomicAdd(counters + 3, (unsigned long long)nfl);
-    if (threadIdx.x == 0 && n_done) atomicAdd(agg + 2, (unsigned long long)n_done);
+    if ((t & 31) == 0 && nfl) atomicAdd(counters + 3, (unsigned long long)nfl);
+    if (t == 0 && n_done) atomicAdd(agg + 2, (unsigned long long)n_done);
 }
 
 // ---- fallback: the global scratch table ------------------------------------------------------------------------------
@@ -1492,6 +1607,22 @@ static uint64_t links_hot_records(int64_t n_used, int bucket_log) {
     return (uint64_t)HH_AGG_HOT * (mean > HH_AGG_MEAN / 2 ? mean : HH_AGG_MEAN / 2);
 }
 
+// hh_k_bucket_count for keys of 2 kbits bits: 32-bit keys in chunks of 2048 records, 64-bit keys in chunks of 1280 (the
+// shared memory of three CTAs per SM)
+template <typename K, int ITEMS>
+static int links_bucket_count(hh_links* lk, const int4* rec, const int64_t* boff, int nb, uint64_t hot, int kbits, uint32_t* compact,
+                              uint64_t compact_cap, unsigned long long* agg, uint32_t* fallback) {
+    hh_ctx* ctx = lk->ctx;
+    auto kernel = hh_k_bucket_count<K, ITEMS>;
+    const size_t smem = sizeof(hh_bc_smem<K, ITEMS>);
+    HH_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int grid = 0;
+    HH_CHECK(hh_resident_grid(ctx, kernel, HH_AGG_THREADS, smem, &grid));
+    HH_LAUNCH(ctx, kernel, grid, HH_AGG_THREADS, smem, rec, boff, nb, hot, kbits, compact, compact_cap, lk->d_ctg, lk->d_counters, agg,
+              fallback);
+    return HH_OK;
+}
+
 // Device memory of the finish for P records sent, U of them usable: the regions (24 B x P + 32 MB at 512 partitions) and
 // the spill list (2 B x P + 64 MB), the bucket buffer (16 B x U) and the compact staging list (36 B x U).  The regions and
 // the spill list are released before the staging list is allocated, so at most 8.7 GB is in use at once at the
@@ -1560,12 +1691,10 @@ static int links_finish_partitioned(hh_links* lk) {
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 0, 0, sizeof(unsigned long long), ctx->stream));     // entry cursor
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));     // nnz_flank
         // ---- every bucket in shared memory
-        const size_t smem = (size_t)HH_AGG_SLOTS * (sizeof(uint64_t) + 7 * sizeof(uint32_t));
-        HH_CUDA(cudaFuncSetAttribute(hh_k_bucket_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int grid_agg = 0;
-        HH_CHECK(hh_resident_grid(ctx, hh_k_bucket_count, HH_AGG_THREADS, smem, &grid_agg));
-        HH_LAUNCH(ctx, hh_k_bucket_count, grid_agg, HH_AGG_THREADS, smem, d_rec2, d_boff, nb, hot, d_stage_compact,
-                  compact_cap, lk->d_ctg, lk->d_counters, d_agg, d_fallback);
+        int kbits = 1;                                         // key (i << kbits) | j
+        while ((1ll << kbits) < (int64_t)lk->n_ctg) kbits++;
+        auto count = 2 * kbits <= 32 ? links_bucket_count<uint32_t, 8> : links_bucket_count<uint64_t, 5>;
+        HH_CHECK(count(lk, d_rec2, d_boff, nb, hot, kbits, d_stage_compact, compact_cap, d_agg, d_fallback));
         unsigned long long agg[4];
         HH_CUDA(cudaMemcpyAsync(agg, d_agg, sizeof(agg), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CHECK(links_read_counters(lk, c));
