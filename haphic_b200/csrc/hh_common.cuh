@@ -154,6 +154,16 @@ __device__ __forceinline__ unsigned long long hh_warp_sum(unsigned long long v) 
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(HH_FULL_MASK, v, o);
     return v;
 }
+// inclusive prefix sum over the lanes of a warp: lane i gets v(0) + ... + v(i)
+template <typename T>
+__device__ __forceinline__ T hh_warp_incl_scan(T v) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T t = __shfl_up_sync(HH_FULL_MASK, v, o);
+        if (hh_lane() >= o) v += t;
+    }
+    return v;
+}
 __device__ __forceinline__ float hh_warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(HH_FULL_MASK, v, o));

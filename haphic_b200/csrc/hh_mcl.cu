@@ -13,7 +13,9 @@
 // ascending i -- no atomics, and the fp32 sums are bit-reproducible for any grid size or GPU count.
 // The epilogue (inflate -> column L1 -> prune/keep-max -> column L1 -> convergence) runs on
 // the accumulator in place and writes the pruned column straight into its slot: the unpruned
-// product never reaches HBM.
+// product never reaches HBM.  The rule of that epilogue is defined once (hh_x1, hh_prune_stats, hh_prune_plan,
+// hh_conv_term below) and used per element by every kernel that prunes: hh_k_col, hh_k_col_win and hh_k_col_small, and
+// for its survivor test and first maximum by hh_k_iter0.
 //
 //   SRC_CSC     scatter an unsorted CSC column            (dict_to_matrix output, 366-368)
 //   SRC_PRODUCT expansion, A.B column product             (mkl_matrix_power, 2017-2023)
@@ -52,6 +54,87 @@ __device__ __forceinline__ float hh_inflate(float x, float rf, int mode) {
         case HH_INFL_X25: return (x * x) * __fsqrt_rn(x);
         default: return powf(x, rf);
     }
+}
+
+// ---------------------------------------------------------------------------------------------
+// The per-column prune rule (1987-2014) and convergence term (2045), shared by every iteration kernel.  Each kernel walks
+// its own storage (accumulator rows, window rows, a merged list) and calls these per element, so the fp64 sums keep the
+// kernel's per-lane order and reduction tree.
+// ---------------------------------------------------------------------------------------------
+// first maximum across the warp: the largest v, ties to the lowest *key; k travels with its v (without key, k is its own key)
+__device__ __forceinline__ void hh_warp_argmax(float& v, int& k, int* key = nullptr) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(HH_FULL_MASK, v, o);
+        const int ok = __shfl_xor_sync(HH_FULL_MASK, k, o);
+        const int okey = key ? __shfl_xor_sync(HH_FULL_MASK, *key, o) : ok;
+        const bool take = ov > v || (ov == v && okey < (key ? *key : k));
+        v = take ? ov : v;
+        k = take ? ok : k;
+        if (key) *key = take ? okey : *key;
+    }
+}
+
+// E2: x1 = fp32(fp64(y) / S1) (a column summing to 0 keeps y)
+__device__ __forceinline__ float hh_x1(float y, double S1) { return (S1 != 0.0) ? (float)((double)y / S1) : y; }
+
+// survivor of the prune: x1 >= pruning; a zero never survives, whatever the threshold
+__device__ __forceinline__ bool hh_survives(float x1, float p32) { return x1 >= p32 && x1 > 0.f; }
+
+// |M - L| - 1e-5 |L| in fp32 with non-contracted operations (2045)
+__device__ __forceinline__ float hh_conv_term(float m, float l) { return __fsub_rn(fabsf(__fsub_rn(m, l)), __fmul_rn(1e-5f, fabsf(l))); }
+
+// what E3 does with a column: its survivors normalised again, or its first maximum alone when nothing survives (2009-2013)
+struct hh_prune_plan {
+    bool need_max;
+    int total;      // entries the column keeps
+    int kmax;       // row of the first maximum
+    float p32;
+    double S2;      // fp64 sum of the survivors
+    __device__ __forceinline__ bool keeps(float x1, int k) const { return need_max ? k == kmax : hh_survives(x1, p32); }
+    // the kept maximum is x1 / x1 = 1
+    __device__ __forceinline__ float x2(float x1) const { return need_max ? 1.0f : (float)((double)x1 / S2); }
+};
+
+// E2 statistics of one lane (or, reduced, of a warp): survivor count and fp64 sum, and the first maximum -- ties go to the
+// lowest ORIGINAL row, so the result does not depend on the relabelling
+struct hh_prune_stats {
+    double s2 = 0.0;
+    int cnt = 0;
+    float vmax = 0.f;
+    int kmax = 0x7fffffff, omax = 0x7fffffff;   // omax: original row of kmax
+    // x1 of row k; a lane sees its rows in ascending order, and orig[] is read only for a new maximum or a tie
+    __device__ __forceinline__ void see(float x1, int k, float p32, const int* orig) {
+        if (hh_survives(x1, p32)) {
+            cnt++;
+            s2 += (double)x1;
+        }
+        if (x1 > vmax || (x1 == vmax && x1 > 0.f)) {
+            const int o = orig ? orig[k] : k;
+            if (x1 > vmax || o < omax) {
+                vmax = x1;
+                kmax = k;
+                omax = o;
+            }
+        }
+    }
+    __device__ __forceinline__ void warp_reduce() {
+        s2 = hh_warp_sum(s2);
+        cnt = hh_warp_sum(cnt);
+        hh_warp_argmax(vmax, kmax, &omax);
+    }
+    // of the reduced statistics of the whole column
+    __device__ __forceinline__ hh_prune_plan plan(float p32) const {
+        const bool need_max = (cnt == 0) && (vmax > 0.f);
+        return hh_prune_plan{need_max, need_max ? 1 : cnt, kmax, p32, s2};
+    }
+};
+
+// the end of writing column j's slot: its last row-block pointer and its length (clamped to the slot), overflow flagged
+__device__ __forceinline__ void hh_slot_close(const hh_slotmat& out, int j, int W, int total, int* err) {
+    out.blk[(size_t)j * (W + 1) + W] = min(total, out.cap);
+    out.len[j] = min(total, out.cap);
+    if (total > out.cap) atomicExch(err, 1);
 }
 
 enum { SRC_CSC = 0, SRC_PRODUCT = 1 };
@@ -278,12 +361,7 @@ __global__ void __launch_bounds__(W * 32) hh_k_col(const hh_colargs a) {
                 const unsigned c_base = __shfl_sync(HH_FULL_MASK, seg_base, src);
                 const float c_v = __shfl_sync(HH_FULL_MASK, seg_v, src);
                 if (lane >= nseg) c_len = 0;
-                int incl = c_len;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const int tt = __shfl_up_sync(HH_FULL_MASK, incl, o);
-                    if (lane >= o) incl += tt;
-                }
+                const int incl = hh_warp_incl_scan(c_len);
                 const int excl = incl - c_len;
                 const int total = __shfl_sync(HH_FULL_MASK, incl, 31);
                 warp_prod += (unsigned long long)total;
@@ -384,12 +462,7 @@ __global__ void __launch_bounds__(W * 32) hh_k_col(const hh_colargs a) {
             const double sv = (lane < W) ? s_d[lane] : 0.0;
             const int cv = (lane < W) ? s_c[lane] : 0;
             const double S = hh_warp_sum(sv);
-            int incl = cv;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int tt = __shfl_up_sync(HH_FULL_MASK, incl, o);
-                if (lane >= o) incl += tt;
-            }
+            const int incl = hh_warp_incl_scan(cv);
             const int base = __shfl_sync(HH_FULL_MASK, incl - cv, w);
             const int total = __shfl_sync(HH_FULL_MASK, incl, 31);
             int off = base;
@@ -409,9 +482,7 @@ __global__ void __launch_bounds__(W * 32) hh_k_col(const hh_colargs a) {
             })
             if (lane == 0) a.out.blk[(size_t)j * (W + 1) + w] = base;
             if (threadIdx.x == 0) {
-                a.out.blk[(size_t)j * (W + 1) + W] = min(total, a.out.cap);
-                a.out.len[j] = min(total, a.out.cap);
-                if (total > a.out.cap) atomicExch(a.err, 1);
+                hh_slot_close(a.out, j, W, total, a.err);
                 nnz_acc += (unsigned long long)total;
             }
         } else {
@@ -434,116 +505,62 @@ __global__ void __launch_bounds__(W * 32) hh_k_col(const hh_colargs a) {
             __syncthreads();   // s_d is reused below
             // E2: normalise, threshold statistics, first maximum
             const float p32 = a.prune;
-            double s2 = 0.0;
-            int cnt = 0;
-            float vbest = 0.f;
-            int kbest = 0x7fffffff, obest = 0x7fffffff;     // obest: ORIGINAL row index of kbest (first maximum = lowest original row)
+            hh_prune_stats st;
             HH_FOR_DIRTY_ROWS({
                 const float y = acc[k];
                 if (y != 0.f) {
-                    const float x1 = (S1 != 0.0) ? (float)((double)y / S1) : y;
+                    const float x1 = hh_x1(y, S1);
                     acc[k] = x1;
-                    if (x1 >= p32 && x1 > 0.f) {
-                        cnt++;
-                        s2 += (double)x1;
-                    }
-                    if (x1 > vbest) {
-                        vbest = x1;
-                        kbest = k;
-                        obest = a.orig ? a.orig[k] : k;
-                    } else if (x1 == vbest && a.orig) {
-                        const int o = a.orig[k];
-                        if (o < obest) {
-                            kbest = k;
-                            obest = o;
-                        }
-                    }
+                    st.see(x1, k, p32, a.orig);
                 }
             })
-            s2 = hh_warp_sum(s2);
-            cnt = hh_warp_sum(cnt);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(HH_FULL_MASK, vbest, o);
-                const int ok = __shfl_xor_sync(HH_FULL_MASK, kbest, o);
-                const int oo = __shfl_xor_sync(HH_FULL_MASK, obest, o);
-                if (ov > vbest || (ov == vbest && oo < obest)) {
-                    vbest = ov;
-                    kbest = ok;
-                    obest = oo;
-                }
-            }
+            st.warp_reduce();
             if (lane == 0) {
-                s_d[w] = s2;
-                s_c[w] = cnt;
-                s_f[w] = vbest;
-                s_k[w] = kbest;
-                s_o[w] = obest;
+                s_d[w] = st.s2;
+                s_c[w] = st.cnt;
+                s_f[w] = st.vmax;
+                s_k[w] = st.kmax;
+                s_o[w] = st.omax;
             }
             __syncthreads();
-            const double sv = (lane < W) ? s_d[lane] : 0.0;
             const int cv = (lane < W) ? s_c[lane] : 0;
-            float vmax = (lane < W) ? s_f[lane] : 0.f;
-            int kmax = (lane < W) ? s_k[lane] : 0x7fffffff;
-            int omax = (lane < W) ? s_o[lane] : 0x7fffffff;
-            double S2 = hh_warp_sum(sv);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(HH_FULL_MASK, vmax, o);
-                const int ok = __shfl_xor_sync(HH_FULL_MASK, kmax, o);
-                const int oo = __shfl_xor_sync(HH_FULL_MASK, omax, o);
-                if (ov > vmax || (ov == vmax && oo < omax)) {
-                    vmax = ov;
-                    kmax = ok;
-                    omax = oo;
-                }
+            hh_prune_stats cs;      // of the whole column
+            if (lane < W) {
+                cs.s2 = s_d[lane];
+                cs.cnt = cv;
+                cs.vmax = s_f[lane];
+                cs.kmax = s_k[lane];
+                cs.omax = s_o[lane];
             }
-            int incl = cv;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int tt = __shfl_up_sync(HH_FULL_MASK, incl, o);
-                if (lane >= o) incl += tt;
-            }
-            int base = __shfl_sync(HH_FULL_MASK, incl - cv, w);
-            int total = __shfl_sync(HH_FULL_MASK, incl, 31);
-            // keep the column maximum when nothing reaches the threshold (2009-2013)
-            const bool need_max = (total == 0) && (vmax > 0.f);
-            if (need_max) {
-                const int wk = kmax / T;
-                base = (w > wk) ? 1 : 0;
-                total = 1;
-                S2 = (double)vmax;
-            }
+            cs.warp_reduce();
+            const hh_prune_plan pl = cs.plan(p32);
+            // first output position of this warp's row block: its survivors follow those of the warps before it
+            int base = __shfl_sync(HH_FULL_MASK, hh_warp_incl_scan(cv) - cv, w);
+            if (pl.need_max) base = (w > pl.kmax / T) ? 1 : 0;
             // E3: compact the survivors in row order, second normalisation (2014)
             int off = base;
             uint2* __restrict__ oent = a.out.ent + (size_t)j * (size_t)a.out.cap;
             const bool conv = a.do_conv != 0;
             HH_FOR_DIRTY_ROWS({
                 const float x1 = acc[k];
-                const bool f = need_max ? (k == kmax) : (x1 >= p32 && x1 > 0.f);
+                const bool f = pl.keeps(x1, k);
                 const unsigned bal = __ballot_sync(HH_FULL_MASK, f);
                 float keepv = 0.f;
                 if (f) {
                     const int pos = off + __popc(bal & lt_mask);
-                    // the kept maximum of a column without survivors is x1 / x1 = 1 (S2 = its own x1)
-                    const float x2 = need_max ? 1.0f : (float)((double)x1 / S2);
-                    if (pos < a.out.cap) {
-                        oent[pos] = make_uint2((unsigned)k, __float_as_uint(x2));
-                    }
-                    keepv = x2;
+                    keepv = pl.x2(x1);
+                    if (pos < a.out.cap) oent[pos] = make_uint2((unsigned)k, __float_as_uint(keepv));
                 }
                 if (x1 != 0.f) acc[k] = conv ? keepv : 0.f;
                 off += __popc(bal);
             })
             if (lane == 0) a.out.blk[(size_t)j * (W + 1) + w] = base;
             if (threadIdx.x == 0) {
-                a.out.blk[(size_t)j * (W + 1) + W] = min(total, a.out.cap);
-                a.out.len[j] = min(total, a.out.cap);
-                if (total > a.out.cap) atomicExch(a.err, 1);
-                nnz_acc += (unsigned long long)total;
+                hh_slot_close(a.out, j, W, pl.total, a.err);
+                nnz_acc += (unsigned long long)pl.total;
             }
             if (SRC == SRC_PRODUCT && conv) {
-                // E4: entries of the previous iterate L = B[:, j]  ->  |M - L| - 1e-5|L|  (fp32, 2045)
+                // E4: entries of the previous iterate L = B[:, j]
                 __syncwarp();
                 const hh_slotmat& Lm = a.use_prev ? a.prev : a.B;
                 const int* bp = Lm.blk + (size_t)j * (W + 1) + w;
@@ -552,10 +569,7 @@ __global__ void __launch_bounds__(W * 32) hh_k_col(const hh_colargs a) {
                 for (int p = ps + lane; p < pe; p += 32) {
                     const uint2 le = Lent[p];
                     const int k = (int)le.x;
-                    const float l = __uint_as_float(le.y);
-                    const float m = acc[k];
-                    const float d = __fsub_rn(fabsf(__fsub_rn(m, l)), __fmul_rn(1e-5f, fabsf(l)));
-                    dmax = fmaxf(dmax, d);
+                    dmax = fmaxf(dmax, hh_conv_term(acc[k], __uint_as_float(le.y)));
                     acc[k] = 0.f;
                 }
                 __syncwarp();
@@ -733,6 +747,43 @@ __global__ void hh_k_cc_lists(const int* __restrict__ perm, int col_lo, int ncol
     else big_list[atomicAdd(counts + 1, 1)] = j;
 }
 
+// Ordered compaction of a component window, rows [lo, lo + width), into column j's slot by one warp.  keep(r, x) says whether
+// row lo + r is kept and sets its value x; it is called once for every row of the window.  Rows ascend, so the row-block
+// pointers are set as the rows pass each boundary.  Returns the number of rows kept.
+template <typename F>
+__device__ __forceinline__ int hh_win_compact(const hh_slotmat& out, int j, int W, int T, int lo, int width, F&& keep) {
+    const int lane = hh_lane();
+    const unsigned lt_mask = (1u << lane) - 1u;
+    uint2* __restrict__ oent = out.ent + (size_t)j * (size_t)out.cap;
+    int* __restrict__ oblk = out.blk + (size_t)j * (W + 1);
+    int bnext = 0;                       // next row-block boundary (row bnext*T) whose pointer is still unset
+    int off = 0;
+    for (int r0 = 0; r0 < width; r0 += 32) {
+        const int r = r0 + lane;
+        float x = 0.f;
+        const bool f = (r < width) && keep(r, x);
+        const unsigned bal = __ballot_sync(HH_FULL_MASK, f);
+        // boundaries that fall at or before the end of this 32-row step
+        while (bnext < W && (long long)bnext * T <= (long long)(lo + r0 + 31)) {
+            const long long brow = (long long)bnext * T;
+            // survivors of this step with row < brow
+            const int nlt = (brow <= lo + r0) ? 0 : (int)(brow - (lo + r0));     // lanes [0, nlt) have row < brow
+            const unsigned below = (nlt >= 32) ? 0xFFFFFFFFu : ((1u << nlt) - 1u);
+            if (lane == 0) oblk[bnext] = min(off + __popc(bal & below), out.cap);
+            bnext++;
+        }
+        if (f) {
+            const int pos = off + __popc(bal & lt_mask);
+            if (pos < out.cap) oent[pos] = make_uint2((unsigned)(lo + r), __float_as_uint(x));
+        }
+        off += __popc(bal);
+    }
+    if (lane == 0) {
+        for (; bnext < W; ++bnext) oblk[bnext] = min(off, out.cap);   // boundaries beyond the window
+    }
+    return off;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Windowed expansion (perm space): ONE WARP per column with a private accumulator of the column's row
 // window (its component).  The warp walks the column's entries in order and streams every operand column
@@ -746,7 +797,6 @@ __global__ void __launch_bounds__(32) hh_k_col_win(const hh_colargs a, int W, co
                                                    const int* __restrict__ comp_lo, const int* __restrict__ comp_hi, int wmax) {
     extern __shared__ __align__(16) float acc[];      // wmax floats, zero between columns
     const int lane = threadIdx.x;
-    const unsigned lt_mask = (1u << lane) - 1u;
     const uint2* __restrict__ Aent = a.A.ent;
     const size_t capA = (size_t)a.A.cap;
     const float p32 = a.prune, rf = a.inflation;
@@ -817,83 +867,30 @@ __global__ void __launch_bounds__(32) hh_k_col_win(const hh_colargs a, int W, co
         }
         const double S1 = hh_warp_sum(s1);
         __syncwarp();
-        // ---- E2: normalise, threshold statistics, first maximum (lowest ORIGINAL row among ties)
-        double s2 = 0.0;
-        int cnt = 0, kmax = 0x7fffffff, omax = 0x7fffffff;
-        float vmax = 0.f;
+        // ---- E2: normalise, threshold statistics, first maximum
+        hh_prune_stats st;
         for (int r = lane; r < width; r += 32) {
             const float y = acc[r];
             if (y != 0.f) {
-                const float x1 = (S1 != 0.0) ? (float)((double)y / S1) : y;
+                const float x1 = hh_x1(y, S1);
                 acc[r] = x1;
-                if (x1 >= p32 && x1 > 0.f) {
-                    cnt++;
-                    s2 += (double)x1;
-                }
-                if (x1 > vmax || (x1 == vmax && x1 > 0.f)) {
-                    const int o = a.orig ? a.orig[lo + r] : (lo + r);
-                    if (x1 > vmax || o < omax) {
-                        vmax = x1;
-                        kmax = lo + r;
-                        omax = o;
-                    }
-                }
+                st.see(x1, lo + r, p32, a.orig);
             }
         }
-        double S2 = hh_warp_sum(s2);
-        cnt = hh_warp_sum(cnt);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(HH_FULL_MASK, vmax, o);
-            const int ok = __shfl_xor_sync(HH_FULL_MASK, kmax, o);
-            const int oo = __shfl_xor_sync(HH_FULL_MASK, omax, o);
-            if (ov > vmax || (ov == vmax && oo < omax)) {
-                vmax = ov;
-                kmax = ok;
-                omax = oo;
-            }
-        }
-        const bool need_max = (cnt == 0) && (vmax > 0.f);
-        int total = cnt;
-        if (need_max) {
-            total = 1;
-            S2 = (double)vmax;
-        }
+        st.warp_reduce();
+        const hh_prune_plan pl = st.plan(p32);
         __syncwarp();
-        // ---- E3: ordered compaction into the slot; row-block pointers on the fly (rows ascend)
-        uint2* __restrict__ oent = a.out.ent + (size_t)j * (size_t)a.out.cap;
-        int* __restrict__ oblk = a.out.blk + (size_t)j * (W + 1);
-        int bnext = 0;                       // next row-block boundary (row bnext*T) whose pointer is still unset
-        int off = 0;
-        for (int r0 = 0; r0 < width; r0 += 32) {
-            const int r = r0 + lane;
-            const float x1 = (r < width) ? acc[r] : 0.f;
-            const bool f = (r < width) && (need_max ? (lo + r == kmax) : (x1 >= p32 && x1 > 0.f));
-            const unsigned bal = __ballot_sync(HH_FULL_MASK, f);
-            // boundaries that fall at or before the end of this 32-row step
-            while (bnext <= W && (long long)bnext * T <= (long long)(lo + r0 + 31)) {
-                const long long brow = (long long)bnext * T;
-                // survivors of this step with row < brow
-                const int nlt = (brow <= lo + r0) ? 0 : (int)(brow - (lo + r0));     // lanes [0, nlt) have row < brow
-                const unsigned below = (nlt >= 32) ? 0xFFFFFFFFu : ((1u << nlt) - 1u);
-                if (lane == 0) oblk[bnext] = min(off + __popc(bal & below), a.out.cap);
-                bnext++;
-            }
-            float keepv = 0.f;
-            if (f) {
-                const int pos = off + __popc(bal & lt_mask);
-                const float x2 = (float)((double)x1 / S2);
-                if (pos < a.out.cap) oent[pos] = make_uint2((unsigned)(lo + r), __float_as_uint(x2));
-                keepv = x2;
-            }
-            if (r < width) acc[r] = conv ? keepv : 0.f;
-            off += __popc(bal);
-        }
+        // ---- E3: ordered compaction into the slot
+        hh_win_compact(a.out, j, W, T, lo, width, [&](int r, float& x2) {
+            const float x1 = acc[r];
+            const bool f = pl.keeps(x1, lo + r);
+            x2 = f ? pl.x2(x1) : 0.f;
+            acc[r] = conv ? x2 : 0.f;
+            return f;
+        });
         if (lane == 0) {
-            for (; bnext <= W; ++bnext) oblk[bnext] = min(total, a.out.cap);   // boundaries beyond the window
-            a.out.len[j] = min(total, a.out.cap);
-            if (total > a.out.cap) atomicExch(a.err, 1);
-            nnz_acc += (unsigned long long)total;
+            hh_slot_close(a.out, j, W, pl.total, a.err);
+            nnz_acc += (unsigned long long)pl.total;
         }
         __syncwarp();
         if (conv) {
@@ -901,9 +898,8 @@ __global__ void __launch_bounds__(32) hh_k_col_win(const hh_colargs a, int W, co
             for (int p = lane; p < lenB; p += 32) {
                 const uint2 le = Bent[p];
                 const unsigned r = le.x - (unsigned)lo;
-                const float l = __uint_as_float(le.y);
                 const float m = (r < (unsigned)width) ? acc[r] : 0.f;
-                dmax = fmaxf(dmax, __fsub_rn(fabsf(__fsub_rn(m, l)), __fmul_rn(1e-5f, fabsf(l))));
+                dmax = fmaxf(dmax, hh_conv_term(m, __uint_as_float(le.y)));
                 if (r < (unsigned)width) acc[r] = 0.f;
             }
             __syncwarp();
@@ -934,7 +930,6 @@ __global__ void __launch_bounds__(32) hh_k_relabel_win(const hh_slotmat src, con
                                                        const int* __restrict__ comp_hi, int wmax, int* __restrict__ err) {
     extern __shared__ __align__(16) float acc[];      // wmax floats, zero between columns
     const int lane = threadIdx.x;
-    const unsigned lt_mask = (1u << lane) - 1u;
     for (int k = lane; k < wmax; k += 32) acc[k] = 0.f;
     __syncwarp();
     for (int jj = blockIdx.x; jj < nlist; jj += gridDim.x) {
@@ -950,32 +945,14 @@ __global__ void __launch_bounds__(32) hh_k_relabel_win(const hh_slotmat src, con
             else atomicExch(err, 2);
         }
         __syncwarp();
-        uint2* __restrict__ oent = out.ent + (size_t)j * (size_t)out.cap;
-        int* __restrict__ oblk = out.blk + (size_t)j * (W + 1);
-        int bnext = 0, off = 0;
-        for (int r0 = 0; r0 < width; r0 += 32) {
-            const int r = r0 + lane;
-            const float x = (r < width) ? acc[r] : 0.f;
-            const bool f = x != 0.f;
-            const unsigned bal = __ballot_sync(HH_FULL_MASK, f);
-            while (bnext <= W && (long long)bnext * T <= (long long)(lo + r0 + 31)) {
-                const long long brow = (long long)bnext * T;
-                const int nlt = (brow <= lo + r0) ? 0 : (int)(brow - (lo + r0));
-                const unsigned below = (nlt >= 32) ? 0xFFFFFFFFu : ((1u << nlt) - 1u);
-                if (lane == 0) oblk[bnext] = min(off + __popc(bal & below), out.cap);
-                bnext++;
-            }
-            if (f) {
-                const int pos = off + __popc(bal & lt_mask);
-                if (pos < out.cap) oent[pos] = make_uint2((unsigned)(lo + r), __float_as_uint(x));
-                acc[r] = 0.f;
-            }
-            off += __popc(bal);
-        }
+        const int total = hh_win_compact(out, j, W, T, lo, width, [&](int r, float& x) {
+            x = acc[r];
+            acc[r] = 0.f;
+            return x != 0.f;
+        });
         if (lane == 0) {
-            for (; bnext <= W; ++bnext) oblk[bnext] = min(off, out.cap);
-            out.len[j] = min(off, out.cap);
-            if (off > out.cap || off != L) atomicExch(err, 1);
+            hh_slot_close(out, j, W, total, err);
+            if (total != L) atomicExch(err, 1);
         }
         __syncwarp();
     }
@@ -1081,47 +1058,18 @@ __global__ void __launch_bounds__(256) hh_k_col_small(const hh_colargs a, int W,
         const double S1 = hh_warp_sum(s1);
         __syncwarp();
         // ---- E2: normalise, threshold statistics, first maximum
-        double s2 = 0.0;
-        int cnt = 0, kmax = 0x7fffffff, omax = 0x7fffffff;
-        float vmax = 0.f;
+        hh_prune_stats st;
         for (int p = lane; p < nout; p += 32) {
             const float y = sv[p];
             if (y != 0.f) {
-                const float x1 = (S1 != 0.0) ? (float)((double)y / S1) : y;
+                const float x1 = hh_x1(y, S1);
                 sv[p] = x1;
-                if (x1 >= p32 && x1 > 0.f) {
-                    cnt++;
-                    s2 += (double)x1;
-                }
-                if (x1 > vmax || (x1 == vmax && x1 > 0.f)) {
-                    const int o = a.orig ? a.orig[sk[p]] : sk[p];      // first maximum = lowest ORIGINAL row
-                    if (x1 > vmax || o < omax) {
-                        vmax = x1;
-                        kmax = sk[p];
-                        omax = o;
-                    }
-                }
+                st.see(x1, sk[p], p32, a.orig);
             }
         }
-        double S2 = hh_warp_sum(s2);
-        cnt = hh_warp_sum(cnt);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(HH_FULL_MASK, vmax, o);
-            const int ok = __shfl_xor_sync(HH_FULL_MASK, kmax, o);
-            const int oo = __shfl_xor_sync(HH_FULL_MASK, omax, o);
-            if (ov > vmax || (ov == vmax && oo < omax)) {
-                vmax = ov;
-                kmax = ok;
-                omax = oo;
-            }
-        }
-        const bool need_max = (cnt == 0) && (vmax > 0.f);
-        int total = cnt;
-        if (need_max) {
-            total = 1;
-            S2 = (double)vmax;
-        }
+        st.warp_reduce();
+        const hh_prune_plan pl = st.plan(p32);
+        const int total = pl.total;
         __syncwarp();
         // ---- E3: ordered compaction (in place in shared memory) + slot write
         uint2* __restrict__ oent = a.out.ent + (size_t)j * (size_t)a.out.cap;
@@ -1130,12 +1078,12 @@ __global__ void __launch_bounds__(256) hh_k_col_small(const hh_colargs a, int W,
             const int p = p0 + lane;
             const float x1 = (p < nout) ? sv[p] : 0.f;
             const int k = (p < nout) ? sk[p] : 0;
-            const bool f = (p < nout) && (need_max ? (k == kmax && x1 > 0.f) : (x1 >= p32 && x1 > 0.f));
+            const bool f = (p < nout) && pl.keeps(x1, k);
             const unsigned bal = __ballot_sync(HH_FULL_MASK, f);
             __syncwarp();
             if (f) {
                 const int pos = off + __popc(bal & lt_mask);
-                const float x2 = (float)((double)x1 / S2);
+                const float x2 = pl.x2(x1);
                 if (pos < a.out.cap) oent[pos] = make_uint2((unsigned)k, __float_as_uint(x2));
                 sk[pos] = k;
                 sv[pos] = x2;
@@ -1155,9 +1103,7 @@ __global__ void __launch_bounds__(256) hh_k_col_small(const hh_colargs a, int W,
             a.out.blk[(size_t)j * (W + 1) + lane] = lo;
         }
         if (lane == 0) {
-            a.out.blk[(size_t)j * (W + 1) + W] = min(total, a.out.cap);
-            a.out.len[j] = min(total, a.out.cap);
-            if (total > a.out.cap) atomicExch(a.err, 1);
+            hh_slot_close(a.out, j, W, total, a.err);
             nnz_acc += (unsigned long long)total;
         }
         // ---- convergence term against the previous iterate L = B[:, j] (its entries sit in the lanes)
@@ -1172,7 +1118,7 @@ __global__ void __launch_bounds__(256) hh_k_col_small(const hh_colargs a, int W,
                     else hi = mid;
                 }
                 const float m = (lo < total && sk[lo] == il) ? sv[lo] : 0.f;
-                dmax = fmaxf(dmax, __fsub_rn(fabsf(__fsub_rn(m, vl)), __fmul_rn(1e-5f, fabsf(vl))));
+                dmax = fmaxf(dmax, hh_conv_term(m, vl));
             }
             for (int p = lane; p < total; p += 32) {
                 const int k = sk[p];
@@ -1225,15 +1171,7 @@ __global__ void hh_k_topn(const hh_slotmat m, int topN, int* __restrict__ top) {
                     bi = i;
                 }
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(HH_FULL_MASK, bv, o);
-                const int oi = __shfl_xor_sync(HH_FULL_MASK, bi, o);
-                if (ov > bv || (ov == bv && oi < bi)) {
-                    bv = ov;
-                    bi = oi;
-                }
-            }
+            hh_warp_argmax(bv, bi);
             int pick;
             if (bv > 0.f) {
                 pick = bi;
@@ -1720,15 +1658,7 @@ __global__ void __launch_bounds__(HH_IT0_WARPS * 32, 32 / HH_IT0_WARPS) hh_k_ite
         __syncthreads();
         // exact x1 of this lane's maximum; two different x may round to one x1: then the lower row wins (first maximum)
         float vbest = (xbest > 0.f && S1 != 0.0) ? hh_it0_x1(xbest, S1, rf, sq) : 0.f;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(HH_FULL_MASK, vbest, o);
-            const int ok = __shfl_xor_sync(HH_FULL_MASK, kbest, o);
-            if (ov > vbest || (ov == vbest && ok < kbest)) {
-                vbest = ov;
-                kbest = ok;
-            }
-        }
+        hh_warp_argmax(vbest, kbest);
         // ---------------------------------------------------------------- pass 2: survivors of the prune, S2
         // x1 >= pruning needs y >= 0.999 * pruning * S1, i.e. x >= (that)^(1/r): taken a little lower, the rest is exact
         const float thr_y = (float)(0.999 * (double)p32 * S1);
@@ -1744,7 +1674,7 @@ __global__ void __launch_bounds__(HH_IT0_WARPS * 32, 32 / HH_IT0_WARPS) hh_k_ite
                     const int i = i0 + lane;
                     if (i < qn) {
                         const float x1 = hh_it0_x1(s_qx[wv][i], S1, rf, sq);
-                        if (x1 >= p32 && x1 > 0.f) {
+                        if (hh_survives(x1, p32)) {
                             cnt++;
                             s2 += (double)x1;
                         }
@@ -1788,21 +1718,8 @@ __global__ void __launch_bounds__(HH_IT0_WARPS * 32, 32 / HH_IT0_WARPS) hh_k_ite
         double S2 = hh_warp_sum((lane < HH_IT0_WARPS) ? s_d[lane] : 0.0);
         float vmax = (lane < HH_IT0_WARPS) ? s_f[lane] : 0.f;
         int kmax = (lane < HH_IT0_WARPS) ? s_k[lane] : 0x7fffffff;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(HH_FULL_MASK, vmax, o);
-            const int ok = __shfl_xor_sync(HH_FULL_MASK, kmax, o);
-            if (ov > vmax || (ov == vmax && ok < kmax)) {
-                vmax = ov;
-                kmax = ok;
-            }
-        }
-        int incl = cv;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int tt = __shfl_up_sync(HH_FULL_MASK, incl, o);
-            if (lane >= o) incl += tt;
-        }
+        hh_warp_argmax(vmax, kmax);
+        const int incl = hh_warp_incl_scan(cv);
         const int excl = incl - cv;                                  // lane b: first output position of row block b
         int total = __shfl_sync(HH_FULL_MASK, incl, 31);
         const bool need_max = (total == 0) && (vmax > 0.f);        // keep the column maximum (2009-2013)
@@ -1830,7 +1747,7 @@ __global__ void __launch_bounds__(HH_IT0_WARPS * 32, 32 / HH_IT0_WARPS) hh_k_ite
                         x1 = hh_it0_x1(s_qx[wv][i], S1, rf, sq);
                         row = s_qr[wv][i];
                     }
-                    const bool sv = (i < qn) && x1 >= p32 && x1 > 0.f;
+                    const bool sv = (i < qn) && hh_survives(x1, p32);
                     const unsigned bal = __ballot_sync(HH_FULL_MASK, sv);
                     if (sv) {
                         const int pos = off + __popc(bal & lt_mask);
@@ -1866,9 +1783,7 @@ __global__ void __launch_bounds__(HH_IT0_WARPS * 32, 32 / HH_IT0_WARPS) hh_k_ite
             if (qn > 0) drain3();
         }
         if (threadIdx.x == 0) {
-            a.out.blk[(size_t)j * (W + 1) + W] = min(total, a.out.cap);
-            a.out.len[j] = min(total, a.out.cap);
-            if (total > a.out.cap) atomicExch(a.err, 1);
+            hh_slot_close(a.out, j, W, total, a.err);
             nnz_acc += (unsigned long long)total;
         }
     }
@@ -1898,29 +1813,23 @@ static int launch_iter0(hh_ctx* ctx, const hh_geom& g, hh_colargs& a) {
     }
 }
 
+// CTAs of the column kernel per SM with the shared-memory accumulator: every instantiation has the same footprint, so the
+// heaviest (product + prune) is queried
+template <int W>
+static int col_per_sm(const hh_geom& g, int* per_sm) {
+    auto kern = hh_k_col<W, SRC_PRODUCT, EPI_PRUNE, true, true, true>;
+    HH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem_bytes));
+    HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, kern, W * 32, g.smem_bytes));
+    return HH_OK;
+}
+
 static int grid_cap_for(hh_ctx* ctx, const hh_geom& g, int* out) {
     int per_sm = 0;
     if (g.smem_acc) {
-        // every instantiation has the same footprint; query the heaviest (product + prune)
         switch (g.W) {
-            case 8:
-                HH_CUDA(cudaFuncSetAttribute(hh_k_col<8, SRC_PRODUCT, EPI_PRUNE, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)g.smem_bytes));
-                HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hh_k_col<8, SRC_PRODUCT, EPI_PRUNE, true, true, true>, 256,
-                                                                     g.smem_bytes));
-                break;
-            case 16:
-                HH_CUDA(cudaFuncSetAttribute(hh_k_col<16, SRC_PRODUCT, EPI_PRUNE, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)g.smem_bytes));
-                HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hh_k_col<16, SRC_PRODUCT, EPI_PRUNE, true, true, true>, 512,
-                                                                     g.smem_bytes));
-                break;
-            default:
-                HH_CUDA(cudaFuncSetAttribute(hh_k_col<32, SRC_PRODUCT, EPI_PRUNE, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)g.smem_bytes));
-                HH_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hh_k_col<32, SRC_PRODUCT, EPI_PRUNE, true, true, true>, 1024,
-                                                                     g.smem_bytes));
-                break;
+            case 8: HH_CHECK(col_per_sm<8>(g, &per_sm)); break;
+            case 16: HH_CHECK(col_per_sm<16>(g, &per_sm)); break;
+            default: HH_CHECK(col_per_sm<32>(g, &per_sm)); break;
         }
     } else {
         per_sm = 2;
@@ -1972,12 +1881,7 @@ hh_k_slot_from_csc(const int64_t* __restrict__ colptr, const int32_t* __restrict
         // exclusive prefix of popc(bm[]) : thread t owns words [t * per, (t + 1) * per)
         uint32_t mine = 0;
         for (int q = 0; q < per; ++q) mine += __popc(bm[tid * per + q]);
-        uint32_t incl = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(HH_FULL_MASK, incl, o);
-            if (lane >= o) incl += t;
-        }
+        const uint32_t incl = hh_warp_incl_scan(mine);
         if (lane == 31) s_wsum[wv] = incl;
         __syncthreads();
         if (tid == 0) {
@@ -2010,14 +1914,11 @@ hh_k_slot_from_csc(const int64_t* __restrict__ colptr, const int32_t* __restrict
                 if ((int)pos < out.cap) oent[pos] = make_uint2(r, __float_as_uint((raw || S == 0.0) ? v : (float)((double)v / S)));
             }
         }
-        for (int w = tid; w <= W; w += 256) {
-            int b = total;
-            if (w < W && w * T < n) b = (int)pre[(w * T) >> 5];        // T is a multiple of 32
-            out.blk[(size_t)j * (W + 1) + w] = (w == W) ? min(total, out.cap) : b;
+        for (int w = tid; w < W; w += 256) {
+            out.blk[(size_t)j * (W + 1) + w] = (w * T < n) ? (int)pre[(w * T) >> 5] : total;        // T is a multiple of 32
         }
         if (tid == 0) {
-            out.len[j] = min(total, out.cap);
-            if (total > out.cap) atomicExch(err, 1);
+            hh_slot_close(out, j, W, total, err);
             nnz_acc += (unsigned long long)total;
         }
         __syncthreads();
