@@ -75,7 +75,13 @@ _SIGNATURES = {
     "hh_links_finish": (C.c_int, [_P, C.POINTER(LinksInfo)]),
     "hh_links_agg_info": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "hh_links_fetch": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
+    "hh_links_fetch_phased": (C.c_int, [_P, _P, C.c_double, _P, _P, _P, _P, C.POINTER(C.c_int64)]),
     "hh_links_fetch_ctg": (C.c_int, [_P, _P]),
+    "hh_stats_create": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, C.c_int64, C.POINTER(_P)]),
+    "hh_stats_rank": (C.c_int, [_P, _P, C.c_int32, C.POINTER(C.c_int64)]),
+    "hh_stats_fetch_ranked": (C.c_int, [_P, _P, _P, _P, _P]),
+    "hh_stats_best": (C.c_int, [_P, _P, C.c_int32, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
+    "hh_stats_destroy": (C.c_int, [_P]),
     "hh_links_export": (C.c_int, [_P, _P, _P]),
     "hh_links_merge": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int64, C.c_int64]),
     "hh_links_route": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int, _P, _P, _P]),

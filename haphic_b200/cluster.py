@@ -14,8 +14,9 @@ Assembly correction (``--correct_nrounds``) runs on the GPU (haphic_b200/correct
 
 ``--gfa`` (hifiasm GFA files, one per haplotype) reads the read depths and haplotypes (parse_gfa): the read-depth filter runs
 in filter_fragments on the host, and with two or more files the inter-haplotype reduction of the flank links
-(reduce_inter_hap_HiC_links) runs inside the device matrix kernels; the contig-level full links are reduced on the fetched
-arrays.  ``--phasing_weight`` must lie in [0, 1].
+(reduce_inter_hap_HiC_links) runs inside the device matrix kernels and the contig-level full links are reduced on the device
+before they are fetched (hh_links_fetch_phased).  After a fractional weight the reassignment statistics sum int / float
+links; they run on the device too (hh_stats).  ``--phasing_weight`` must lie in [0, 1].
 
 Not supported (raise, never silently degrade): ``--ul`` (ignored with a warning together with ``--correct_nrounds``, as
 in the reference).
@@ -148,8 +149,8 @@ def reduce_inter_hap_HiC_links(link_dict, read_depth_dict, phasing_weight, targe
     """695-707: every link between two different haplotypes becomes ``v - v * phasing_weight`` (two roundings) and is
     deleted when that is 0; the other entries keep their order and type.
 
-    ``link_dict`` is the reference's dict (edited in place), a LinkArrays (fp64 pass on the arrays, LinkArrays.reduce_phasing)
-    or the device LinkTable with its fragment ``names``: the flank links then stay on the device and the reduction runs
+    ``link_dict`` is the reference's dict (edited in place), a LinkArrays (fp64 pass on the arrays, LinkArrays.reduce_phasing,
+    unless the device already reduced it when it was fetched: LinkArrays.from_phased) or the device LinkTable with its fragment ``names``: the flank links then stay on the device and the reduction runs
     inside the matrix kernels (hh_matrix_from_links_phased), so this only returns the haplotype array of the table's
     fragments for device_matrix."""
     logger.info("Reducing inter-haplotype Hi-C links in {}...".format(target))
@@ -157,7 +158,8 @@ def reduce_inter_hap_HiC_links(link_dict, read_depth_dict, phasing_weight, targe
     if isinstance(link_dict, LinkTable):
         return haplotype_array(read_depth_dict, names)
     if isinstance(link_dict, LinkArrays):
-        link_dict.reduce_phasing(haplotype_array(read_depth_dict, link_dict.names), phasing_weight)
+        if not link_dict.phased:
+            link_dict.reduce_phasing(haplotype_array(read_depth_dict, link_dict.names), phasing_weight)
         return None
     deleted = []
     for pair, links in link_dict.items():
@@ -985,14 +987,25 @@ class LinkArrays:
     """full_link_dict as the arrays the device table hands out (entry order = dict insertion order): run() keeps the
     links in this form so that no 10^7-entry Python dict is ever built; `to_dict()` gives the reference's object."""
 
-    def __init__(self, names, key_i, key_j, values):
+    def __init__(self, names, key_i, key_j, values, is_float=None):
         self.names = names
         self.key_i = np.ascontiguousarray(key_i, dtype=np.int32)
         self.key_j = np.ascontiguousarray(key_j, dtype=np.int32)
-        self.values = np.ascontiguousarray(values, dtype=np.int64)
         # None: every value is a Python int (int64 values).  Else values are fp64 and is_float[e] says whether entry e is a
         # Python float in the reference's dict (an inter-haplotype link reduced by a fractional phasing weight).
-        self.is_float = None
+        self.is_float = None if is_float is None else np.asarray(is_float, dtype=bool)
+        self.values = np.ascontiguousarray(values, dtype=np.int64 if is_float is None else np.float64)
+        self.phased = False         # reduce_inter_hap_HiC_links has been applied
+        self._stats = None
+
+    @classmethod
+    def from_phased(cls, names, fetched):
+        """The arrays of LinkTable.fetch_phased (reduced on the device).  Without a float among them (w = 1, or one haplotype)
+        the values are ints, as reduce_phasing leaves them."""
+        flt = fetched["is_float"].astype(bool)
+        arr = cls(names, fetched["key_i"], fetched["key_j"], fetched["values"], flt if flt.any() else None)
+        arr.phased = True
+        return arr
 
     def __len__(self):
         return len(self.key_i)
@@ -1015,7 +1028,18 @@ class LinkArrays:
         else:
             self.is_float = inter if self.is_float is None else (self.is_float[keep] | inter)
             self.values = x[keep]
+        self.phased = True
         self._directed = self._directed_dev = None
+        if self._stats is not None:
+            self._stats.close()
+            self._stats = None
+
+    def stats_device(self, ctx):
+        """The int / float links resident on the device for the statistics of every inflation (GroupLinkStats); built once."""
+        if self._stats is None or self._stats.ctx is not ctx:
+            from .links import GroupLinkStats
+            self._stats = GroupLinkStats(ctx, len(self.names), self.key_i, self.key_j, self.values, self.is_float)
+        return self._stats
 
     def directed(self):
         """(L, ctg, other): the symmetric link matrix as CSR (int64 values) and the 2 * nnz directed entries interleaved in the
@@ -1092,10 +1116,17 @@ def _python_numbers(sums, is_float):
     return [v if f else int(v) for v, f in zip(sums.tolist(), is_float.tolist())]
 
 
+def _stats_on_device():
+    """The statistics run on the GPU once a context exists; HAPHIC_STATS_DEVICE=0 keeps them on the host (the reference the
+    tests compare against)."""
+    return _CTX is not None and os.environ.get("HAPHIC_STATS_DEVICE", "1") != "0"
+
+
 def _ranked_group_arrays(link_dict, ctg_group_dict):
     """(gid, contig, group, links, is_float) of the same ranking as flat arrays ordered by (contig, rank); None when nothing
     is linked to a group.  gid[c] = group of contig c (-1 = ungrouped).  is_float is None for integer links; after a
-    fractional phasing weight (LinkArrays.is_float) links are fp64 sums and is_float marks the float-valued ones."""
+    fractional phasing weight (LinkArrays.is_float) links are fp64 sums and is_float marks the float-valued ones; those are
+    ranked on the device (hh_stats_rank) unless the statistics are kept on the host."""
     names = link_dict.names
     n = len(names)
     gid = np.array([-1 if ctg_group_dict[nm] == "ungrouped" else ctg_group_dict[nm] for nm in names], dtype=np.int64)
@@ -1103,8 +1134,13 @@ def _ranked_group_arrays(link_dict, ctg_group_dict):
         return None
     ng = int(gid.max()) + 1
     if link_dict.is_float is not None:
+        if _stats_on_device():
+            st = link_dict.stats_device(_CTX)
+            st.rank(gid, ng)
+            c_of, g_of, sums, is_f = st.fetch_ranked()
+            return gid, c_of.astype(np.int64), g_of.astype(np.int64), sums, is_f
         return (gid,) + _ranked_group_links_mixed(link_dict, gid, ng)
-    if _CTX is not None and os.environ.get("HAPHIC_STATS_DEVICE", "1") != "0":
+    if _stats_on_device():
         return (gid,) + tuple(_ranked_group_links_device(link_dict, gid, ng, _CTX.device)) + (None,)
     # links of every contig into every group = (symmetric link matrix) x (contig -> group indicator): one sparse product per
     # inflation instead of a sort of all 2 * nnz directed entries (20 sorts of 1.2e8 keys took 15 min at 50k contigs)
@@ -1224,6 +1260,8 @@ def _best_group_statistics(fa_dict, link_dict, ctg_group, group_RE):
     arithmetic in the same order: int / int true divisions become float64 divisions of the same integers (both correctly
     rounded), and the sum over ranked[1:] is accumulated position by position, left to right, like sum()."""
     names = link_dict.names
+    if link_dict.is_float is not None and _stats_on_device():
+        return _best_group_statistics_device(fa_dict, link_dict, ctg_group, group_RE)
     arr = _ranked_group_arrays(link_dict, ctg_group)
     zero = [(ctg, 0) for ctg in fa_dict]
     if arr is None:
@@ -1267,6 +1305,38 @@ def _best_group_statistics(fa_dict, link_dict, ctg_group, group_RE):
     for ctg in fa_dict:
         k = has.get(name_idx.get(ctg, -1))
         if k is None:
+            best_links.append((ctg, 0))
+            best_density.append((ctg, 0))
+            best_ratio.append((ctg, 0))
+            continue
+        best_links.append((ctg, top_links[k]))
+        best_density.append((ctg, top_dens[k]))
+        best_ratio.append((ctg, ratio_l[k] if others_l[k] else 1000000))
+    return best_links, best_density, best_ratio
+
+
+def _best_group_statistics_device(fa_dict, link_dict, ctg_group, group_RE):
+    """_best_group_statistics for int / float links on the device (hh_stats_rank, hh_stats_best): the same arithmetic in the
+    same order, and only the per-contig results come back to the host."""
+    names = link_dict.names
+    n_groups = len(group_RE)
+    if n_groups == 0:
+        zero = [(ctg, 0) for ctg in fa_dict]
+        return zero, list(zero), list(zero)
+    gid = np.array([-1 if ctg_group[nm] == "ungrouped" else ctg_group[nm] for nm in names], dtype=np.int32)
+    st = link_dict.stats_device(_CTX)
+    st.rank(gid, n_groups)
+    RE_g = np.array([group_RE[g] for g in range(n_groups)], dtype=np.int64)
+    RE_c = np.array([fa_dict[nm][2] for nm in names], dtype=np.int64)
+    r = st.best(RE_g, RE_c, compensated=sys.version_info >= (3, 12))
+    has = r["has"].astype(bool).tolist()
+    top_links = _python_numbers(r["top_links"], r["top_is_float"].astype(bool))
+    top_dens, others_l, ratio_l = r["top_density"].tolist(), r["others"].tolist(), r["ratio"].tolist()
+    name_idx = {nm: i for i, nm in enumerate(names)}
+    best_links, best_density, best_ratio = [], [], []
+    for ctg in fa_dict:
+        k = name_idx.get(ctg)
+        if k is None or not has[k]:
             best_links.append((ctg, 0))
             best_density.append((ctg, 0))
             best_ratio.append((ctg, 0))
@@ -1562,6 +1632,11 @@ def run(args, log_file=None):
         logger.info("Writing {} to {}...".format("HT_link_dict", "HT_links.pkl"))
         full_link_dict.write_pickle("HT_links.pkl", ht=fetched["ht"])
         del fetched
+        if phasing:
+            # full_link_dict as reduce_inter_hap_HiC_links leaves it (2926-2928), reduced on the device while the contig-level
+            # table is still there; the reduction below then only logs
+            full_link_dict = LinkArrays.from_phased(st["names"], st["table"].fetch_phased(
+                haplotype_array(ctg_read_depth_dict, st["names"]), args.phasing_weight))
         clm_src = (st["clm_rec"], st["names"], st["ctg_len"], st["rank"])
         if split_ctg_set:
             st["table"].close()                         # full / HT links were contig-level; the rest is fragment-level

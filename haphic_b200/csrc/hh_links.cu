@@ -2058,6 +2058,97 @@ extern "C" int hh_links_fetch(hh_links* lk, int32_t* key_i, int32_t* key_j, uint
     return rc;
 }
 
+// The full count of an entry after reduce_inter_hap_HiC_links (695-707): x - x * w in fp64 with two roundings when its ends
+// lie on different haplotypes (then a Python float), else the count (an int).  The same expression as hh_flank_value.
+__device__ __forceinline__ double hh_full_value(const uint32_t* __restrict__ p, const int32_t* __restrict__ hap, double w,
+                                                bool* is_float) {
+    const double x = (double)p[HH_E_FULL];
+    *is_float = hap[p[HH_E_I]] != hap[p[HH_E_J]];
+    return *is_float ? __dsub_rn(x, __dmul_rn(x, w)) : x;
+}
+
+// order[e] = e for the entries that stay (value != 0), HH_NONE32 for the deleted ones; n_kept counts the former
+__global__ void __launch_bounds__(256)
+hh_k_phased_mark(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ hap, double w,
+                 uint32_t* __restrict__ order, unsigned long long* __restrict__ n_kept) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    int kept = 0;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
+        bool f;
+        const bool keep = hh_full_value(compact + e * HH_E_WORDS, hap, w, &f) != 0.0;
+        order[e] = keep ? (uint32_t)e : HH_NONE32;
+        kept += keep;
+    }
+    kept = hh_warp_sum(kept);
+    if ((threadIdx.x & 31) == 0 && kept) atomicAdd(n_kept, (unsigned long long)kept);
+}
+
+// the kept entries -> key_i, key_j, values, is_float (SoA: int32 | int32 | fp64 | uint8 blocks of n)
+__global__ void __launch_bounds__(256)
+hh_k_phased_split(const uint32_t* __restrict__ kept, int64_t n, const int32_t* __restrict__ hap, double w, int32_t* __restrict__ ki,
+                  int32_t* __restrict__ kj, double* __restrict__ val, uint8_t* __restrict__ flt) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
+        const uint32_t* p = kept + e * HH_E_WORDS;
+        bool f;
+        val[e] = hh_full_value(p, hap, w, &f);
+        ki[e] = (int32_t)p[HH_E_I];
+        kj[e] = (int32_t)p[HH_E_J];
+        flt[e] = f;
+    }
+}
+
+extern "C" int hh_links_fetch_phased(hh_links* lk, const int32_t* hap, double w, int32_t* key_i, int32_t* key_j, double* values,
+                                     uint8_t* is_float, int64_t* n_out) {
+    HH_REQUIRE(lk && hap && key_i && key_j && values && is_float && n_out, HH_ERR_ARG, "hh_links_fetch_phased: NULL argument");
+    HH_REQUIRE(w >= 0.0 && w <= 1.0, HH_ERR_ARG, "hh_links_fetch_phased: phasing weight %g outside [0, 1]", w);
+    hh_scope _scope(lk->ctx);
+    HH_REQUIRE(lk->finished, HH_ERR_STATE, "hh_links_fetch_phased: call hh_links_finish first");
+    *n_out = 0;
+    if (lk->nnz == 0) return HH_OK;
+    hh_ctx* ctx = lk->ctx;
+    HH_CHECK(links_order_list(lk));
+    const int64_t nnz = lk->nnz;
+    int32_t* d_hap = nullptr;
+    uint32_t *d_order = nullptr, *d_kept = nullptr;
+    uint8_t* d_soa = nullptr;
+    unsigned long long* d_n = nullptr;
+    const int rc = [&]() -> int {
+        HH_CHECK(hh_dmalloc(&d_hap, (size_t)lk->n_ctg));
+        HH_CHECK(hh_dmalloc(&d_order, (size_t)nnz));
+        HH_CHECK(hh_dmalloc(&d_n, 1));
+        HH_CUDA(cudaMemcpyAsync(d_hap, hap, (size_t)lk->n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+        HH_CUDA(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), ctx->stream));
+        HH_LAUNCH(ctx, hh_k_phased_mark, links_grid(ctx, nnz), 256, 0, lk->d_compact, nnz, d_hap, w, d_order, d_n);
+        unsigned long long n_kept = 0;
+        HH_CUDA(cudaMemcpyAsync(&n_kept, d_n, sizeof(n_kept), cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaStreamSynchronize(ctx->stream));
+        const int64_t n = (int64_t)n_kept;
+        *n_out = n;
+        if (n == 0) return HH_OK;
+        // stable: the kept entries stay in dict insertion order
+        HH_CHECK(hh_dmalloc(&d_kept, (size_t)n * HH_E_WORDS));
+        HH_CHECK(links_compact(lk, d_order, nnz, nullptr, reinterpret_cast<const hh_slot*>(lk->d_compact), d_kept));
+        HH_CHECK(hh_dmalloc(&d_soa, (size_t)n * 17));
+        int32_t* ki = reinterpret_cast<int32_t*>(d_soa);
+        double* val = reinterpret_cast<double*>(d_soa + (size_t)n * 8);
+        uint8_t* flt = d_soa + (size_t)n * 16;
+        HH_LAUNCH(ctx, hh_k_phased_split, links_grid(ctx, n), 256, 0, d_kept, n, d_hap, w, ki, ki + n, val, flt);
+        HH_CUDA(cudaMemcpyAsync(key_i, ki, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaMemcpyAsync(key_j, ki + n, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaMemcpyAsync(values, val, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaMemcpyAsync(is_float, flt, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaStreamSynchronize(ctx->stream));
+        return HH_OK;
+    }();
+    hh_dfree(d_hap);
+    hh_dfree(d_order);
+    hh_dfree(d_kept);
+    hh_dfree(d_soa);
+    hh_dfree(d_n);
+    return rc;
+}
+
 extern "C" int hh_links_fetch_ctg(hh_links* lk, int64_t* ctg_links) {
     HH_REQUIRE(lk && ctg_links, HH_ERR_ARG, "hh_links_fetch_ctg: NULL argument");
     HH_CUDA(cudaSetDevice(lk->ctx->device));

@@ -137,6 +137,21 @@ class LinkTable:
                                     ptr(out["first_full"]), ptr(out["first_flank"]), ptr(out["ht"])))
         return out
 
+    def fetch_phased(self, hap, phasing_weight: float) -> dict:
+        """full_link_dict after reduce_inter_hap_HiC_links (695-707) with ``hap`` (haplotype index per contig), reduced on the
+        device (hh_links_fetch_phased): key_i, key_j, fp64 values and is_float (uint8) of the entries that remain, in dict
+        insertion order."""
+        if self.info is None:
+            self.finish()
+        hap = self._hap(hap)
+        nnz = int(self.info.nnz_full)
+        out = {"key_i": np.empty(nnz, np.int32), "key_j": np.empty(nnz, np.int32), "values": np.empty(nnz, np.float64),
+               "is_float": np.empty(nnz, np.uint8)}
+        n = C.c_int64()
+        check(load().hh_links_fetch_phased(self._h, ptr(hap), float(phasing_weight), ptr(out["key_i"]), ptr(out["key_j"]),
+                                           ptr(out["values"]), ptr(out["is_float"]), C.byref(n)))
+        return {k: v[:int(n.value)] for k, v in out.items()}
+
     def fetch_ctg(self) -> np.ndarray:
         tot = np.empty(self.n_ctg, np.int64)
         check(load().hh_links_fetch_ctg(self._h, ptr(tot)))
@@ -291,6 +306,70 @@ class LinkMatrix:
     def close(self):
         if self._h:
             load().hh_matrix_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class GroupLinkStats:
+    """Full links with Python floats among them, resident on the device for the reassignment statistics of every inflation
+    (hh_stats): parse_link_dict's (contig, group) sums, their ranking and the best-group statistics of output_statistics."""
+
+    _close_order = 1
+
+    def __init__(self, ctx: Context, n_ctg: int, key_i, key_j, values, is_float):
+        self.ctx = ctx
+        self.n_ctg = int(n_ctg)
+        ki = np.ascontiguousarray(key_i, dtype=np.int32)
+        kj = np.ascontiguousarray(key_j, dtype=np.int32)
+        v = np.ascontiguousarray(values, dtype=np.float64)
+        f = np.ascontiguousarray(is_float, dtype=np.uint8)
+        m = len(ki)
+        self._h = C.c_void_p()
+        check(load().hh_stats_create(ctx.handle, self.n_ctg, ptr(ki) if m else None, ptr(kj) if m else None, ptr(v) if m else None,
+                                     ptr(f) if m else None, m, C.byref(self._h)))
+        ctx.adopt(self)
+        self.n_ranked = 0
+
+    def rank(self, group, n_groups: int) -> int:
+        """Rank every contig's groups (``group`` per contig, -1 = ungrouped, else < n_groups); returns the number of sums."""
+        g = np.ascontiguousarray(group, dtype=np.int32)
+        if g.shape != (self.n_ctg,):
+            raise ValueError("group must have one entry per contig")
+        n = C.c_int64()
+        check(load().hh_stats_rank(self._h, ptr(g), int(n_groups), C.byref(n)))
+        self.n_ranked = int(n.value)
+        return self.n_ranked
+
+    def fetch_ranked(self):
+        """(contig, group, links, is_float) of the last ranking, ordered by (contig, rank)."""
+        n = self.n_ranked
+        c, g = np.empty(n, np.int32), np.empty(n, np.int32)
+        s, f = np.empty(n, np.float64), np.empty(n, np.uint8)
+        check(load().hh_stats_fetch_ranked(self._h, ptr(c), ptr(g), ptr(s), ptr(f)))
+        return c, g, s, f.astype(bool)
+
+    def best(self, group_re, ctg_re, compensated: bool) -> dict:
+        """Per contig over the last ranking: has, top_links, top_is_float, top_density, others, ratio (hh_stats_best)."""
+        gre = np.ascontiguousarray(group_re, dtype=np.int64)
+        cre = np.ascontiguousarray(ctg_re, dtype=np.int64)
+        if cre.shape != (self.n_ctg,):
+            raise ValueError("ctg_re must have one entry per contig")
+        n = self.n_ctg
+        out = {"has": np.empty(n, np.uint8), "top_links": np.empty(n, np.float64), "top_is_float": np.empty(n, np.uint8),
+               "top_density": np.empty(n, np.float64), "others": np.empty(n, np.float64), "ratio": np.empty(n, np.float64)}
+        check(load().hh_stats_best(self._h, ptr(gre), len(gre), ptr(cre), int(bool(compensated)), ptr(out["has"]),
+                                   ptr(out["top_links"]), ptr(out["top_is_float"]), ptr(out["top_density"]), ptr(out["others"]),
+                                   ptr(out["ratio"])))
+        return out
+
+    def close(self):
+        if self._h:
+            load().hh_stats_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

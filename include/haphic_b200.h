@@ -120,6 +120,13 @@ int hh_links_agg_info(hh_links* lk, int64_t* buckets, int64_t* smem_buckets, int
  * ti/tj = 1 for the `_T` half (`coord*2 > len`, 404-416).  Any pointer may be NULL. */
 int hh_links_fetch(hh_links* lk, int32_t* key_i, int32_t* key_j, uint32_t* full, uint32_t* flank,
                    uint32_t* first_full, uint32_t* first_flank, uint32_t* ht);
+/* full_link_dict after reduce_inter_hap_HiC_links (695-707, --gfa with >= 2 haplotype files): hap[n_ctg] (host) is the
+ * haplotype index of every contig, w in [0, 1] the phasing weight.  An entry whose ends differ in hap becomes x - x * w
+ * (fp64, two roundings, x = the full count) and is a Python float (is_float = 1); the others keep their count (is_float = 0).
+ * Entries that become exactly 0 are deleted; the rest keep dict insertion order.  The outputs are host buffers of nnz_full
+ * entries, of which the first *n_out are written. */
+int hh_links_fetch_phased(hh_links* lk, const int32_t* hap, double w, int32_t* key_i, int32_t* key_j, double* values,
+                          uint8_t* is_float, int64_t* n_out);
 /* ctg_link_dict (1638-1639): per-contig flank-link totals, [n_ctg] */
 int hh_links_fetch_ctg(hh_links* lk, int64_t* ctg_links);
 /* multi-GPU: export the finished table as device arrays / merge a peer's export into this
@@ -182,6 +189,32 @@ int hh_matrix_info(hh_matrix* m, int32_t* n, int64_t* nnz);
 /* canonical CSC (row-sorted) of the raw link matrix, host buffers: indptr[n+1], indices/data[nnz] */
 int hh_matrix_fetch_csc(hh_matrix* m, int64_t* indptr, int32_t* indices, float* data);
 int hh_matrix_destroy(hh_matrix* m);
+
+/* ---- reassignment statistics over int / float full links: output_statistics, HapHiC_cluster.py:2279-2478 ------------
+ * For full links with Python floats among them (after a fractional phasing weight); every result is the reference's fp64
+ * arithmetic in the reference's order, bit for bit.
+ *   hh_stats_create: the full links (n_entries in dict insertion order, values exact integers or floats, is_float per
+ *     entry), kept on the device for every later call.  n_entries < 2^30.
+ *   hh_stats_rank: parse_link_dict (2245-2258) and the ranking of 2373 for group[n_ctg] (host; -1 = ungrouped, else
+ *     < n_groups): the links of every contig into every group, summed by sequential fp64 adds in the order parse_link_dict
+ *     visits them (first end of entry 0, second end of entry 0, first end of entry 1, ...), a sum being a float iff one of
+ *     its links is; each contig's groups ranked by sum descending, ties by the first visit.  *n_ranked = number of
+ *     (contig, group) sums.
+ *   hh_stats_fetch_ranked: those sums in (contig, rank) order, host buffers of n_ranked entries (any may be NULL).
+ *   hh_stats_best: the three per-contig quantities of 2373-2400 over the last ranking, host buffers of n_ctg entries:
+ *     has = the contig has a ranked list; top_links / top_is_float = links to the first group; top_density =
+ *     cal_link_density to it; others = the sum of the densities of the other ranked groups in rank order (CPython >= 3.12
+ *     sum() with its Neumaier compensation when `compensated`, else plain adds) / (n_groups - 1), 0 when n_groups == 1;
+ *     ratio = top_density / others (inf or nan when others == 0).  group_re[n_groups] = RE sites of every group,
+ *     ctg_re[n_ctg] = RE sites of every contig. */
+typedef struct hh_stats hh_stats;
+int hh_stats_create(hh_ctx* ctx, int32_t n_ctg, const int32_t* key_i, const int32_t* key_j, const double* values,
+                    const uint8_t* is_float, int64_t n_entries, hh_stats** out);
+int hh_stats_rank(hh_stats* st, const int32_t* group, int32_t n_groups, int64_t* n_ranked);
+int hh_stats_fetch_ranked(hh_stats* st, int32_t* ctg, int32_t* group, double* links, uint8_t* is_float);
+int hh_stats_best(hh_stats* st, const int64_t* group_re, int32_t n_groups, const int64_t* ctg_re, int compensated, uint8_t* has,
+                  double* top_links, uint8_t* top_is_float, double* top_density, double* others, double* ratio);
+int hh_stats_destroy(hh_stats* st);
 
 /* ---- Markov clustering: run_mcl_clustering / mcl / prune, HapHiC_cluster.py:1987-2062, 2132-2162
  * hh_mcl_create does 2144 (column-L1 normalise, M0) and 2146-2149 (pre-expansion M1 = M0^e, kept
