@@ -15,8 +15,11 @@ Assembly correction (``--correct_nrounds``) runs on the GPU (haphic_b200/correct
 ``--gfa`` (hifiasm GFA files, one per haplotype) reads the read depths and haplotypes (parse_gfa): the read-depth filter runs
 in filter_fragments on the host, and with two or more files the inter-haplotype reduction of the flank links
 (reduce_inter_hap_HiC_links) runs inside the device matrix kernels and the contig-level full links are reduced on the device
-before they are fetched (hh_links_fetch_phased).  After a fractional weight the reassignment statistics sum int / float
-links; they run on the device too (hh_stats).  ``--phasing_weight`` must lie in [0, 1].
+before they are fetched (hh_links_fetch_phased).  ``--phasing_weight`` must lie in [0, 1].
+
+The reassignment statistics of every inflation (output_statistics) run on the device (hh_stats) for every form of the full
+links: integer counts, ints and floats after a fractional phasing weight, and the host-edited dict of the
+``--remove_allelic_links`` / ``--remove_concentrated_links`` runs.
 
 Not supported (raise, never silently degrade): ``--ul`` (ignored with a warning together with ``--correct_nrounds``, as
 in the reference).
@@ -149,17 +152,17 @@ def reduce_inter_hap_HiC_links(link_dict, read_depth_dict, phasing_weight, targe
     """695-707: every link between two different haplotypes becomes ``v - v * phasing_weight`` (two roundings) and is
     deleted when that is 0; the other entries keep their order and type.
 
-    ``link_dict`` is the reference's dict (edited in place), a LinkArrays (fp64 pass on the arrays, LinkArrays.reduce_phasing,
-    unless the device already reduced it when it was fetched: LinkArrays.from_phased) or the device LinkTable with its fragment ``names``: the flank links then stay on the device and the reduction runs
-    inside the matrix kernels (hh_matrix_from_links_phased), so this only returns the haplotype array of the table's
-    fragments for device_matrix."""
+    ``link_dict`` is the reference's dict (edited in place), a LinkArrays that the device already reduced when it was fetched
+    (LinkArrays.from_phased; this then only logs) or the device LinkTable with its fragment ``names``: the flank links then
+    stay on the device and the reduction runs inside the matrix kernels (hh_matrix_from_links_phased), so this only returns
+    the haplotype array of the table's fragments for device_matrix."""
     logger.info("Reducing inter-haplotype Hi-C links in {}...".format(target))
     from .links import LinkTable
     if isinstance(link_dict, LinkTable):
         return haplotype_array(read_depth_dict, names)
     if isinstance(link_dict, LinkArrays):
         if not link_dict.phased:
-            link_dict.reduce_phasing(haplotype_array(read_depth_dict, link_dict.names), phasing_weight)
+            raise ValueError("full links as arrays are reduced when they are fetched (LinkTable.fetch_phased)")
         return None
     deleted = []
     for pair, links in link_dict.items():
@@ -972,17 +975,6 @@ def add_ungrouped_ctgs(fa_dict, ctg_group_dict):
         ctg_group_dict.setdefault(ctg, "ungrouped")
 
 
-def parse_link_dict(link_dict, ctg_group_dict):
-    out = defaultdict(dict)
-    for (ci, cj), links in link_dict.items():
-        gi, gj = ctg_group_dict[ci], ctg_group_dict[cj]
-        if gj != "ungrouped":
-            out[ci][gj] = out[ci].get(gj, 0) + links
-        if gi != "ungrouped":
-            out[cj][gi] = out[cj].get(gi, 0) + links
-    return out
-
-
 class LinkArrays:
     """full_link_dict as the arrays the device table hands out (entry order = dict insertion order): run() keeps the
     links in this form so that no 10^7-entry Python dict is ever built; `to_dict()` gives the reference's object."""
@@ -992,81 +984,43 @@ class LinkArrays:
         self.key_i = np.ascontiguousarray(key_i, dtype=np.int32)
         self.key_j = np.ascontiguousarray(key_j, dtype=np.int32)
         # None: every value is a Python int (int64 values).  Else values are fp64 and is_float[e] says whether entry e is a
-        # Python float in the reference's dict (an inter-haplotype link reduced by a fractional phasing weight).
+        # Python float in the reference's dict (an inter-haplotype link reduced by a fractional phasing weight, or a scaled one).
         self.is_float = None if is_float is None else np.asarray(is_float, dtype=bool)
         self.values = np.ascontiguousarray(values, dtype=np.int64 if is_float is None else np.float64)
-        self.phased = False         # reduce_inter_hap_HiC_links has been applied
+        self.phased = False         # reduce_inter_hap_HiC_links has been applied (on the device, from_phased)
         self._stats = None
 
     @classmethod
     def from_phased(cls, names, fetched):
         """The arrays of LinkTable.fetch_phased (reduced on the device).  Without a float among them (w = 1, or one haplotype)
-        the values are ints, as reduce_phasing leaves them."""
+        the values are ints, as reduce_inter_hap_HiC_links leaves them."""
         flt = fetched["is_float"].astype(bool)
         arr = cls(names, fetched["key_i"], fetched["key_j"], fetched["values"], flt if flt.any() else None)
         arr.phased = True
         return arr
 
+    @classmethod
+    def from_dict(cls, names, link_dict):
+        """The reference's full_link_dict as arrays over ``names`` (the contigs in fa_dict order), entries in insertion order.
+        An entry is a float iff its value is a Python float, integral ones included (5.0 from ``v - v * 0.0`` or ``*= 1.0``);
+        is_float is None when no value is."""
+        index = {nm: i for i, nm in enumerate(names)}
+        n = len(link_dict)
+        ki = np.fromiter((index[a] for a, _ in link_dict), np.int32, n)
+        kj = np.fromiter((index[b] for _, b in link_dict), np.int32, n)
+        values = list(link_dict.values())
+        is_float = np.fromiter((isinstance(v, float) for v in values), bool, n)
+        return cls(names, ki, kj, values, is_float if is_float.any() else None)
+
     def __len__(self):
         return len(self.key_i)
 
-    def reduce_phasing(self, hap, phasing_weight):
-        """reduce_inter_hap_HiC_links (695-707) on the arrays: entries between haplotypes (``hap`` per contig) become
-        v - v * w in fp64 (two roundings, as Python evaluates it), zeros are dropped, the order is kept.  With w = 1 every
-        such entry is dropped and the values stay integers."""
-        inter = hap[self.key_i] != hap[self.key_j]
-        if not inter.any():
-            return
-        x = self.values.astype(np.float64)
-        xi = x[inter]
-        x[inter] = xi - xi * float(phasing_weight)
-        keep = x != 0
-        self.key_i, self.key_j = self.key_i[keep], self.key_j[keep]
-        inter = inter[keep]
-        if self.is_float is None and not inter.any():
-            self.values = self.values[keep]
-        else:
-            self.is_float = inter if self.is_float is None else (self.is_float[keep] | inter)
-            self.values = x[keep]
-        self.phased = True
-        self._directed = self._directed_dev = None
-        if self._stats is not None:
-            self._stats.close()
-            self._stats = None
-
     def stats_device(self, ctx):
-        """The int / float links resident on the device for the statistics of every inflation (GroupLinkStats); built once."""
+        """The links resident on the device for the statistics of every inflation (GroupLinkStats); built once."""
         if self._stats is None or self._stats.ctx is not ctx:
             from .links import GroupLinkStats
             self._stats = GroupLinkStats(ctx, len(self.names), self.key_i, self.key_j, self.values, self.is_float)
         return self._stats
-
-    def directed(self):
-        """(L, ctg, other): the symmetric link matrix as CSR (int64 values) and the 2 * nnz directed entries interleaved in the
-        order parse_link_dict (2245-2258) visits them (first end of entry 0, second end of entry 0, first end of entry 1,
-        ...); built once, shared by every inflation's statistics."""
-        if getattr(self, "_directed", None) is None:
-            import scipy.sparse as sp
-            n = len(self.names)
-            ctg = np.empty(2 * len(self.key_i), np.int32)
-            oth = np.empty(2 * len(self.key_i), np.int32)
-            ctg[0::2], ctg[1::2] = self.key_i, self.key_j
-            oth[0::2], oth[1::2] = self.key_j, self.key_i
-            L = sp.csr_matrix((np.repeat(self.values, 2), (ctg, oth)), shape=(n, n))
-            self._directed = (L, ctg, oth)
-        return self._directed
-
-    def directed_device(self, dev):
-        """The interleaved directed entries as int64 CUDA tensors (contig, other end, links); built once."""
-        if getattr(self, "_directed_dev", None) is None or self._directed_dev[0].device != dev:
-            import torch
-            ki = torch.from_numpy(self.key_i).to(dev).to(torch.int64)
-            kj = torch.from_numpy(self.key_j).to(dev).to(torch.int64)
-            v = torch.from_numpy(self.values).to(dev)
-            ctg = torch.stack([ki, kj], dim=1).reshape(-1)
-            oth = torch.stack([kj, ki], dim=1).reshape(-1)
-            self._directed_dev = (ctg, oth, torch.stack([v, v], dim=1).reshape(-1))
-        return self._directed_dev
 
     def to_dict(self):
         d = defaultdict(int)
@@ -1077,9 +1031,7 @@ class LinkArrays:
 
     def python_values(self):
         """The values as the reference's dict holds them: ints, and floats where is_float."""
-        if self.is_float is None:
-            return self.values.tolist()
-        return [v if f else int(v) for v, f in zip(self.values.tolist(), self.is_float.tolist())]
+        return _python_numbers(self.values, self.is_float)
 
     def write_pickle(self, path, ht=None):
         """full_links.pkl (or HT_links.pkl when the [n, 4] HT counters are given) with the native writer."""
@@ -1097,18 +1049,6 @@ class LinkArrays:
                                      ptr(np.ascontiguousarray(ht, dtype=np.uint32)) if ht is not None else None))
 
 
-def ranked_group_links(link_dict, ctg_group_dict):
-    """For every contig with links to grouped contigs: [(group, links), ...] ranked by links descending, ties in the
-    order parse_link_dict (2245-2258) first meets the group -- what output_statistics sorts out of it (2373)."""
-    if not isinstance(link_dict, LinkArrays):
-        return {ctg: sorted(groups.items(), key=lambda x: x[1], reverse=True)
-                for ctg, groups in parse_link_dict(link_dict, ctg_group_dict).items()}
-    arr = _ranked_group_arrays(link_dict, ctg_group_dict)
-    if arr is None:
-        return {}
-    return _ranked_lists(link_dict.names, *arr[1:])
-
-
 def _python_numbers(sums, is_float):
     """Sums as the reference's dict values: ints, or floats where any contributing link was a float."""
     if is_float is None:
@@ -1116,218 +1056,22 @@ def _python_numbers(sums, is_float):
     return [v if f else int(v) for v, f in zip(sums.tolist(), is_float.tolist())]
 
 
-def _stats_on_device():
-    """The statistics run on the GPU once a context exists; HAPHIC_STATS_DEVICE=0 keeps them on the host (the reference the
-    tests compare against)."""
-    return _CTX is not None and os.environ.get("HAPHIC_STATS_DEVICE", "1") != "0"
-
-
-def _ranked_group_arrays(link_dict, ctg_group_dict):
-    """(gid, contig, group, links, is_float) of the same ranking as flat arrays ordered by (contig, rank); None when nothing
-    is linked to a group.  gid[c] = group of contig c (-1 = ungrouped).  is_float is None for integer links; after a
-    fractional phasing weight (LinkArrays.is_float) links are fp64 sums and is_float marks the float-valued ones; those are
-    ranked on the device (hh_stats_rank) unless the statistics are kept on the host."""
-    names = link_dict.names
-    n = len(names)
-    gid = np.array([-1 if ctg_group_dict[nm] == "ungrouped" else ctg_group_dict[nm] for nm in names], dtype=np.int64)
-    if len(link_dict) == 0 or gid.max() < 0:
-        return None
-    ng = int(gid.max()) + 1
-    if link_dict.is_float is not None:
-        if _stats_on_device():
-            st = link_dict.stats_device(_CTX)
-            st.rank(gid, ng)
-            c_of, g_of, sums, is_f = st.fetch_ranked()
-            return gid, c_of.astype(np.int64), g_of.astype(np.int64), sums, is_f
-        return (gid,) + _ranked_group_links_mixed(link_dict, gid, ng)
-    if _stats_on_device():
-        return (gid,) + tuple(_ranked_group_links_device(link_dict, gid, ng, _CTX.device)) + (None,)
-    # links of every contig into every group = (symmetric link matrix) x (contig -> group indicator): one sparse product per
-    # inflation instead of a sort of all 2 * nnz directed entries (20 sorts of 1.2e8 keys took 15 min at 50k contigs)
-    import scipy.sparse as sp
-    L, ctg_dir, oth_dir = link_dict.directed()
-    grouped = np.nonzero(gid >= 0)[0]
-    G = sp.csr_matrix((np.ones(len(grouped), np.int64), (grouped, gid[grouped])), shape=(n, ng))
-    S = sp.csr_matrix(L @ G)
-    S.eliminate_zeros()
-    c_of = np.repeat(np.arange(n, dtype=np.int64), np.diff(S.indptr))
-    g_of = S.indices.astype(np.int64)
-    sums = S.data.astype(np.int64)
-    # ties between groups of one contig are ranked by where parse_link_dict first meets the group, i.e. by the smallest
-    # position in the interleaved list (first end of entry 0, second end of entry 0, first end of entry 1, ...).  Only the
-    # contigs that have such a tie need it: their directed entries are written into a (tie rows x groups) table in DESCENDING
-    # position order, so the smallest position is what remains (one pass, no sort).
-    first = np.zeros(len(sums), np.int64)
-    pre = np.lexsort((-sums, c_of))
-    cs, ss = c_of[pre], sums[pre]
-    tie = np.zeros(n, bool)
-    eq = (cs[1:] == cs[:-1]) & (ss[1:] == ss[:-1])
-    tie[cs[1:][eq]] = True
-    if tie.any():
-        nt = int(tie.sum())
-        trow = np.full(n, nt, np.int64)                            # contigs without a tie share one dump row
-        trow[tie] = np.arange(nt)
-        g_oth = gid[oth_dir]
-        key = trow[ctg_dir] * ng + np.where(g_oth >= 0, g_oth, 0)
-        key[g_oth < 0] = nt * ng                                   # links to ungrouped contigs: into the dump row as well
-        tab = np.full((nt + 1) * ng, -1, np.int64)
-        tab[key[::-1]] = np.arange(len(key) - 1, -1, -1, dtype=np.int64)
-        mine = np.nonzero(tie[c_of])[0]
-        first[mine] = tab[trow[c_of[mine]] * ng + g_of[mine]]
-    rank = np.lexsort((first, -sums, c_of))
-    return gid, c_of[rank], g_of[rank], sums[rank], None
-
-
-def _ranked_group_links_mixed(link_dict, gid, ng):
-    """The ranking for int / float links.  parse_link_dict (2245-2258) adds a contig's links to one group one by one in its
-    visiting order, starting from int 0: integer prefixes are exact in fp64, so plain sequential fp64 adds in that order give
-    its sums, and a sum is a float iff one of its links is.  The adds run position by position across all (contig, group)
-    segments at once, longest segments first, so every step works on a prefix of the segments."""
-    m = len(link_dict)
-    ctg = np.empty(2 * m, np.int64)
-    oth = np.empty(2 * m, np.int64)
-    ctg[0::2], ctg[1::2] = link_dict.key_i, link_dict.key_j
-    oth[0::2], oth[1::2] = link_dict.key_j, link_dict.key_i
-    g = gid[oth]
-    pos = np.nonzero(g >= 0)[0]                                 # position in the visiting order
-    if len(pos) == 0:
-        z = np.zeros(0, np.int64)
-        return z, z, np.zeros(0, np.float64), np.zeros(0, bool)
-    key = ctg[pos] * ng + g[pos]
-    order = np.argsort(key, kind="stable")                     # by key, then by position
-    ks = key[order]
-    val = np.repeat(link_dict.values, 2)[pos][order]
-    flt = np.repeat(link_dict.is_float, 2)[pos][order]
-    starts = np.concatenate([[0], np.nonzero(np.diff(ks))[0] + 1])
-    seg_len = np.diff(np.concatenate([starts, [len(ks)]]))
-    by_len = np.argsort(-seg_len, kind="stable")
-    st_sorted, len_sorted = starts[by_len], seg_len[by_len]
-    acc = np.zeros(len(starts), np.float64)
-    for p in range(int(len_sorted[0])):
-        k = int(np.searchsorted(-len_sorted, -p, side="left"))   # segments longer than p: a prefix
-        acc[:k] += val[st_sorted[:k] + p]
-    sums = np.empty(len(starts), np.float64)
-    sums[by_len] = acc
-    is_f = np.logical_or.reduceat(flt, starts)
-    first = pos[order][starts]                                  # first position of each segment
-    c_of, g_of = ks[starts] // ng, ks[starts] % ng
-    rank = np.lexsort((first, -sums, c_of))
-    return c_of[rank], g_of[rank], sums[rank], is_f[rank]
-
-
-def _ranked_lists(names, c_of, g_of, sums, is_float=None):
-    """{contig: [(group, links), ...]} from arrays already ordered by (contig, rank)."""
-    if len(c_of) == 0:
-        return {}
-    cuts = np.concatenate([[0], np.nonzero(np.diff(c_of))[0] + 1, [len(c_of)]])
-    out = {}
-    g_list, s_list = g_of.tolist(), _python_numbers(sums, is_float)
-    for k in range(len(cuts) - 1):
-        lo, hi = int(cuts[k]), int(cuts[k + 1])
-        out[names[int(c_of[lo])]] = list(zip(g_list[lo:hi], s_list[lo:hi]))
-    return out
-
-
-def _ranked_group_links_device(link_dict, gid, ng, device):
-    """The same ranking with the 2 * nnz directed entries resident on the GPU (torch tensor ops as plumbing: gather, unique,
-    integer index_add, scatter-min, stable sorts; integer arithmetic only, so the result is the numpy path's bit for bit)."""
-    import torch
-    dev = device if isinstance(device, torch.device) else torch.device("cuda", device)
-    ctg, oth, val = link_dict.directed_device(dev)
-    g = torch.from_numpy(gid).to(dev)[oth]
-    idx = torch.nonzero(g >= 0).squeeze(1)                   # position in parse_link_dict's visiting order
-    key = ctg[idx] * ng + g[idx]
-    uk, inv = torch.unique(key, return_inverse=True)
-    sums = torch.zeros(len(uk), dtype=torch.int64, device=dev).index_add_(0, inv, val[idx])
-    first = torch.full((len(uk),), 1 << 62, dtype=torch.int64, device=dev).scatter_reduce_(0, inv, idx, "amin", include_self=True)
-    c_of = torch.div(uk, ng, rounding_mode="floor")
-    g_of = uk - c_of * ng
-    o = torch.argsort(first, stable=True)
-    o = o[torch.argsort(-sums[o], stable=True)]
-    o = o[torch.argsort(c_of[o], stable=True)]
-    return c_of[o].cpu().numpy(), g_of[o].cpu().numpy(), sums[o].cpu().numpy()
-
-
-def cal_link_density(max_group, current_group, max_links, group_RE_sites, ctg_RE_sites):
-    if max_group == current_group:
-        return max_links / group_RE_sites
-    return max_links / (group_RE_sites + ctg_RE_sites - 1)
-
-
-def _best_group_statistics(fa_dict, link_dict, ctg_group, group_RE):
-    """The three per-contig lists of output_statistics (2373-2400: links to the best group, link density to it, density ratio
-    best / average of the others) from the ranked (contig, group, links) arrays instead of 10^7 Python tuples.  Same
-    arithmetic in the same order: int / int true divisions become float64 divisions of the same integers (both correctly
-    rounded), and the sum over ranked[1:] is accumulated position by position, left to right, like sum()."""
-    names = link_dict.names
-    if link_dict.is_float is not None and _stats_on_device():
-        return _best_group_statistics_device(fa_dict, link_dict, ctg_group, group_RE)
-    arr = _ranked_group_arrays(link_dict, ctg_group)
-    zero = [(ctg, 0) for ctg in fa_dict]
-    if arr is None:
-        return zero, list(zero), list(zero)
-    gid, c_of, g_of, sums, is_float = arr
-    n_groups = len(group_RE)
-    RE_g = np.array([group_RE[g] for g in range(int(gid.max()) + 1)], dtype=np.int64)
-    RE_c = np.array([fa_dict[nm][2] for nm in names], dtype=np.int64)
-    starts = np.concatenate([[0], np.nonzero(np.diff(c_of))[0] + 1])
-    seg_len = np.diff(np.concatenate([starts, [len(c_of)]]))
-    seg_c = c_of[starts]
-    # per-entry attributes of the entry's contig: c_of is sorted, so np.repeat over the segments replaces two random gathers
-    denom = RE_g[g_of] + np.repeat(RE_c[seg_c] - 1, seg_len)              # cal_link_density: other group
-    same = np.nonzero(g_of == np.repeat(gid[seg_c], seg_len))[0]          # ... the contig's own group (few entries)
-    denom[same] = RE_g[g_of[same]]
-    dens = sums.astype(np.float64) / denom.astype(np.float64)
-    # sum(): left to right; CPython >= 3.12 adds floats with Neumaier's compensated summation (bltinmodule.c), earlier
-    # versions plainly -- the statistics files hold the repr of these sums, so the same algorithm is applied here
-    acc = np.zeros(len(starts), np.float64)
-    comp = np.zeros(len(starts), np.float64)
-    neumaier = sys.version_info >= (3, 12)
-    for pos in range(1, int(seg_len.max())):
-        m = np.nonzero(seg_len > pos)[0]
-        x = dens[starts[m] + pos]
-        f = acc[m]
-        t = f + x
-        if neumaier:
-            comp[m] += np.where(np.abs(f) >= np.abs(x), (f - t) + x, (x - t) + f)
-        acc[m] = t
-    if neumaier:
-        fix = (comp != 0) & np.isfinite(comp)
-        acc[fix] += comp[fix]
-    others = acc / (n_groups - 1) if n_groups > 1 else np.zeros(len(starts))
-    with np.errstate(divide="ignore", invalid="ignore"):
-        ratio = dens[starts] / others
-    has = {int(c): k for k, c in enumerate(c_of[starts].tolist())}
-    top_links, top_dens = _python_numbers(sums[starts], None if is_float is None else is_float[starts]), dens[starts].tolist()
-    others_l, ratio_l = others.tolist(), ratio.tolist()
-    name_idx = {nm: i for i, nm in enumerate(names)}
-    best_links, best_density, best_ratio = [], [], []
-    for ctg in fa_dict:
-        k = has.get(name_idx.get(ctg, -1))
-        if k is None:
-            best_links.append((ctg, 0))
-            best_density.append((ctg, 0))
-            best_ratio.append((ctg, 0))
-            continue
-        best_links.append((ctg, top_links[k]))
-        best_density.append((ctg, top_dens[k]))
-        best_ratio.append((ctg, ratio_l[k] if others_l[k] else 1000000))
-    return best_links, best_density, best_ratio
-
-
-def _best_group_statistics_device(fa_dict, link_dict, ctg_group, group_RE):
-    """_best_group_statistics for int / float links on the device (hh_stats_rank, hh_stats_best): the same arithmetic in the
-    same order, and only the per-contig results come back to the host."""
-    names = link_dict.names
+def _best_group_statistics(fa_dict, links, ctg_group, group_RE):
+    """The three per-contig lists of output_statistics (2355-2391) in fa_dict order: links to the best group, link density
+    to it, density ratio best / average of the others.  parse_link_dict's (contig, group) sums (2252-2268), their ranking
+    and the per-contig results are computed on the device (hh_stats_rank, hh_stats_best) with the reference's fp64
+    arithmetic in its order; only the per-contig results come back."""
+    names = links.names
     n_groups = len(group_RE)
     if n_groups == 0:
         zero = [(ctg, 0) for ctg in fa_dict]
         return zero, list(zero), list(zero)
     gid = np.array([-1 if ctg_group[nm] == "ungrouped" else ctg_group[nm] for nm in names], dtype=np.int32)
-    st = link_dict.stats_device(_CTX)
+    st = links.stats_device(_context())
     st.rank(gid, n_groups)
     RE_g = np.array([group_RE[g] for g in range(n_groups)], dtype=np.int64)
     RE_c = np.array([fa_dict[nm][2] for nm in names], dtype=np.int64)
+    # sum() adds floats with Neumaier's compensation from CPython 3.12 on (bltinmodule.c), plainly before
     r = st.best(RE_g, RE_c, compensated=sys.version_info >= (3, 12))
     has = r["has"].astype(bool).tolist()
     top_links = _python_numbers(r["top_links"], r["top_is_float"].astype(bool))
@@ -1348,7 +1092,10 @@ def _best_group_statistics_device(fa_dict, link_dict, ctg_group, group_RE):
 
 
 def output_statistics(fa_dict, link_dict, result_clusters_list):
+    """2279-2478.  ``link_dict`` is full_link_dict as LinkArrays or as the reference's dict, which is read once into arrays
+    for all inflations and not changed."""
     logger.info("Making some statistics for the next HapHiC reassignment step...")
+    links = link_dict if isinstance(link_dict, LinkArrays) else LinkArrays.from_dict(list(fa_dict), link_dict)
     total_n = len(fa_dict)
     total_len = sum(info[1] for info in fa_dict.values())
 
@@ -1391,30 +1138,7 @@ def output_statistics(fa_dict, link_dict, result_clusters_list):
                 ctg_group[ctg] = gid
                 group_RE[gid] += fa_dict[ctg][2] - 1
         add_ungrouped_ctgs(fa_dict, ctg_group)
-        if isinstance(link_dict, LinkArrays):
-            best_links, best_density, best_ratio = _best_group_statistics(fa_dict, link_dict, ctg_group, group_RE)
-            group_links = None
-        else:
-            group_links = ranked_group_links(link_dict, ctg_group)
-            best_links, best_density, best_ratio = [], [], []
-        for ctg in (fa_dict if group_links is not None else ()):
-            if ctg not in group_links:
-                best_links.append((ctg, 0))
-                best_density.append((ctg, 0))
-                best_ratio.append((ctg, 0))
-                continue
-            ranked = group_links[ctg]
-            top_group, top_links = ranked[0]
-            cur = ctg_group[ctg]
-            ctg_RE = fa_dict[ctg][2]
-            dens = cal_link_density(top_group, cur, top_links, group_RE[top_group], ctg_RE)
-            if len(group_RE) > 1:
-                others = sum(cal_link_density(g, cur, l, group_RE[g], ctg_RE) for g, l in ranked[1:]) / (len(group_RE) - 1)
-            else:
-                others = 0
-            best_links.append((ctg, top_links))
-            best_density.append((ctg, dens))
-            best_ratio.append((ctg, dens / others if others else 1000000))
+        best_links, best_density, best_ratio = _best_group_statistics(fa_dict, links, ctg_group, group_RE)
         curves = {}
         for title, lst in (("Link_threshold", best_links), ("Link_density_threshold", best_density),
                            ("Link_density_ratio_threshold", best_ratio)):

@@ -1,9 +1,11 @@
-// Reassignment statistics over int / float full links (output_statistics, HapHiC_cluster.py:2245-2478, after a fractional
-// --phasing_weight): the (contig, group) link sums that parse_link_dict (2245-2258) accumulates, each contig's groups ranked
-// by them, and the best-group link, density and density ratio.  The statistics files hold the repr of fp64 results, so
-// every sum here is the serial chain of adds the reference makes, in its order:
+// Reassignment statistics over the full links (output_statistics, HapHiC_cluster.py:2245-2478): the (contig, group) link
+// sums that parse_link_dict (2245-2258) accumulates, each contig's groups ranked by them, and the best-group link, density
+// and density ratio.  The links are integer counts, or ints and Python floats after a fractional --phasing_weight or a
+// link scaling.  The statistics files hold the repr of fp64 results, so every sum here is the serial chain of adds the
+// reference makes, in its order:
 //   * a segment (contig, group) is summed with sequential fp64 adds over its directed entries in visiting order, from 0.
-//     Integer prefixes are exact in fp64, so this is Python's int + int / int + float chain bit for bit.
+//     Integer prefixes are exact in fp64 (counts are uint32, every sum stays far below 2^53), so this is Python's
+//     int + int / int + float chain bit for bit.
 //   * `others` adds the densities of ranked[1:] in rank order with CPython >= 3.12 sum()'s Neumaier compensation.
 // No tree reduction: a short chain runs on one lane; a long one (more than 32 terms) on a whole warp, which loads 32 terms
 // at a time and hands them to the accumulator in order through shuffles (every lane carries the same accumulator).

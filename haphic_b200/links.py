@@ -316,19 +316,20 @@ class LinkMatrix:
 
 
 class GroupLinkStats:
-    """Full links with Python floats among them, resident on the device for the reassignment statistics of every inflation
-    (hh_stats): parse_link_dict's (contig, group) sums, their ranking and the best-group statistics of output_statistics."""
+    """The full links, resident on the device for the reassignment statistics of every inflation (hh_stats):
+    parse_link_dict's (contig, group) sums, their ranking and the best-group statistics of output_statistics.  Any form of
+    full_link_dict: integer counts (``is_float`` None), or ints and Python floats (``is_float`` per entry)."""
 
     _close_order = 1
 
-    def __init__(self, ctx: Context, n_ctg: int, key_i, key_j, values, is_float):
+    def __init__(self, ctx: Context, n_ctg: int, key_i, key_j, values, is_float=None):
         self.ctx = ctx
         self.n_ctg = int(n_ctg)
         ki = np.ascontiguousarray(key_i, dtype=np.int32)
         kj = np.ascontiguousarray(key_j, dtype=np.int32)
         v = np.ascontiguousarray(values, dtype=np.float64)
-        f = np.ascontiguousarray(is_float, dtype=np.uint8)
         m = len(ki)
+        f = np.zeros(m, np.uint8) if is_float is None else np.ascontiguousarray(is_float, dtype=np.uint8)
         self._h = C.c_void_p()
         check(load().hh_stats_create(ctx.handle, self.n_ctg, ptr(ki) if m else None, ptr(kj) if m else None, ptr(v) if m else None,
                                      ptr(f) if m else None, m, C.byref(self._h)))

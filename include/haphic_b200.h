@@ -190,9 +190,9 @@ int hh_matrix_info(hh_matrix* m, int32_t* n, int64_t* nnz);
 int hh_matrix_fetch_csc(hh_matrix* m, int64_t* indptr, int32_t* indices, float* data);
 int hh_matrix_destroy(hh_matrix* m);
 
-/* ---- reassignment statistics over int / float full links: output_statistics, HapHiC_cluster.py:2279-2478 ------------
- * For full links with Python floats among them (after a fractional phasing weight); every result is the reference's fp64
- * arithmetic in the reference's order, bit for bit.
+/* ---- reassignment statistics over the full links: output_statistics, HapHiC_cluster.py:2279-2478 ---------------------
+ * For every form of full_link_dict: integer counts (is_float all 0), or ints and Python floats after a fractional phasing
+ * weight or a link scaling; every result is the reference's fp64 arithmetic in the reference's order, bit for bit.
  *   hh_stats_create: the full links (n_entries in dict insertion order, values exact integers or floats, is_float per
  *     entry), kept on the device for every later call.  n_entries < 2^30.
  *   hh_stats_rank: parse_link_dict (2245-2258) and the ranking of 2373 for group[n_ctg] (host; -1 = ungrouped, else

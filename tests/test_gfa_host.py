@@ -1,7 +1,7 @@
 """Host side of `haphic cluster --gfa` against what the unmodified reference computed (tests/golden/gfa_*.npz, made by
 tests/golden/make_gfa_golden.py): parse_gfa and its messages, the read-depth filter of filter_fragments,
-reduce_inter_hap_HiC_links on the frozen dicts (value types included), the fp64 pass of LinkArrays with the full_links.pkl
-writer, and the --phasing_weight range check.  No GPU."""
+reduce_inter_hap_HiC_links on the frozen dicts (value types included), the fp64 pass over the full links' arrays with the
+full_links.pkl writer, and the --phasing_weight range check.  No GPU."""
 
 import json
 import logging
@@ -163,10 +163,12 @@ def test_reduce_inter_hap_links_matches_reference(capture, tag, target):
 
 
 @pytest.mark.parametrize("tag", PHASED)
-def test_link_arrays_reduction_and_pickle_match_reference(tmp_path, tag):
-    """LinkArrays.reduce_phasing (the array path's full_link_dict) gives the reference's dict, and the native writer's
-    full_links.pkl loads as that dict: same order, same values, floats and ints where the reference has them."""
+def test_oracle_reduction_of_arrays_and_pickle_match_reference(tmp_path, tag):
+    """The fp64 reduction of the full links on arrays (tests/stats_oracle.py, the host reference of the device's
+    hh_links_fetch_phased) gives the reference's dict, and the native writer's full_links.pkl loads as that dict: same
+    order, same values, floats and ints where the reference has them."""
     from haphic_b200 import cluster
+    from tests.stats_oracle import reduce_phasing
     import __graft_entry__
     __graft_entry__.build()
     g = load_golden("gfa_{}.npz".format(tag))
@@ -178,7 +180,7 @@ def test_link_arrays_reduction_and_pickle_match_reference(tmp_path, tag):
     ids = {n: i for i, n in enumerate(names)}
     arr = cluster.LinkArrays(names, [ids[a] for a, _ in before], [ids[b] for _, b in before], list(before.values()))
     hap = np.array([red["hap"][n] for n in names], np.int32)
-    arr.reduce_phasing(hap, red["weight"])
+    arr = reduce_phasing(arr, hap, red["weight"])
     assert typed_items(arr.to_dict()) == red["after"]
     want = golden_json(g, "full_links_items")
     assert typed_items(arr.to_dict()) == want

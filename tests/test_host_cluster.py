@@ -322,18 +322,15 @@ def test_allelic_link_removal_matches_reference_golden(tag):
     assert list(full2.items()) == list(full.items()) and list(flank2.items()) == list(flank.items()) and remaining2 == remaining
 
 
-def test_array_backed_links_give_the_same_pickles_and_statistics(tmp_path, monkeypatch):
-    """run() keeps full_link_dict as arrays (LinkArrays): the native pickle loads as the reference's defaultdict and
-    output_statistics writes the same files as from the dict (ties between groups included)."""
+def test_array_backed_links_give_the_same_pickles(tmp_path, monkeypatch):
+    """run() keeps full_link_dict as arrays (LinkArrays): the native pickles load as the reference's defaultdicts."""
     import pickle
     from haphic_b200 import cluster
     g = load_golden("links_b.npz")
     names = g["names"].tolist()
     rng = np.random.default_rng(4)
     ki, kj = g["full_keys"][:, 0], g["full_keys"][:, 1]
-    vals = g["full_vals"].copy()
-    vals[rng.random(len(vals)) < 0.5] = 1                       # plenty of ties between groups
-    la = cluster.LinkArrays(names, ki, kj, vals)
+    la = cluster.LinkArrays(names, ki, kj, g["full_vals"])
     full = la.to_dict()
     monkeypatch.chdir(tmp_path)
     la.write_pickle("full_links.pkl")
@@ -351,18 +348,6 @@ def test_array_backed_links_give_the_same_pickles_and_statistics(tmp_path, monke
             if ht[e, c]:
                 want[(names[a] + "_" + "HT"[c >> 1], names[b] + "_" + "HT"[c & 1])] = int(ht[e, c])
     assert got == want
-    # statistics: random groups of different sizes, some contigs ungrouped
-    fa_dict = {n: [None, int(l), int(r)] for n, l, r in zip(names, g["lengths"].tolist(), g["RE_sites"].tolist())}
-    lab = rng.integers(-1, 5, size=len(names))
-    clusters = [[[n for n, l in zip(names, lab.tolist()) if l == k], 0] for k in range(5)]
-    for tag, links in (("dict", full), ("arrays", la)):
-        os.makedirs(tmp_path / tag / "inflation_1.5")
-        monkeypatch.chdir(tmp_path / tag)
-        cluster.output_statistics(fa_dict, links, [("1.5", clusters)])
-    for fn in sorted(os.listdir(tmp_path / "dict" / "inflation_1.5")):
-        if fn.endswith(".txt"):
-            assert (tmp_path / "dict" / "inflation_1.5" / fn).read_text() == (tmp_path / "arrays" / "inflation_1.5" / fn).read_text(), fn
-    assert len(os.listdir(tmp_path / "arrays" / "inflation_1.5")) >= 4
 
 
 def _python_pairs_reference(text, names, inter_only):
@@ -425,28 +410,51 @@ def test_native_pairs_tokenizer_fuzz_against_python_semantics(tmp_path, seed):
             assert f.read() == want_bed
 
 
-def test_group_link_ranking_on_tensors_equals_the_host_paths():
-    """ranked_group_links has three implementations: the reference's dict walk (parse_link_dict), the numpy / scipy one for
-    array-backed links, and the torch tensor one run() uses on the GPU.  Same ranking from all three, ties between groups
-    included (the tensor version is run on CPU tensors here)."""
-    import torch
+def _typed_ranking(ranked):
+    return {c: [(g, type(v).__name__, repr(v)) for g, v in lst] for c, lst in ranked.items()}
+
+
+def test_group_link_ranking_on_arrays_equals_the_dict_walk():
+    """The array oracle of the reassignment statistics (tests/stats_oracle.py, which the device is compared against at
+    size) ranks every contig's groups as the reference's dict walk does (parse_link_dict, then a stable sort by links
+    descending): same groups, same sums with the same int / float types, ties in first-met order.  The arrays come from
+    the dict by LinkArrays.from_dict, as output_statistics reads a dict."""
     from haphic_b200 import cluster
+    from tests import stats_oracle as so
     rng = np.random.default_rng(3)
     n, m = 1500, 120000
     ki, kj = rng.integers(0, n, m), rng.integers(0, n, m)
     ok = ki < kj
     key = np.unique(ki[ok] * n + kj[ok])
     key = key[rng.permutation(len(key))]
-    ki, kj = key // n, key % n
-    vals = rng.integers(1, 3, len(ki))                          # 1 or 2 links: ties everywhere
+    ki, kj = (key // n).tolist(), (key % n).tolist()
     names = ["ctg{}".format(i) for i in range(n)]
-    la = cluster.LinkArrays(names, ki, kj, vals)
     lab = rng.integers(-1, 25, n)
+    lab[:40] = -1                                               # contigs 0..39 are ungrouped ...
     groups = {nm: (int(g) if g >= 0 else "ungrouped") for nm, g in zip(names, lab.tolist())}
-    from_dict = cluster.ranked_group_links(la.to_dict(), groups)
-    from_arrays = cluster.ranked_group_links(la, groups)
-    gid = np.array([-1 if groups[nm] == "ungrouped" else groups[nm] for nm in names], dtype=np.int64)
-    c, g, s = cluster._ranked_group_links_device(la, gid, int(gid.max()) + 1, torch.device("cpu"))
-    from_tensors = cluster._ranked_lists(names, c, g, s)
-    assert from_arrays == from_dict
-    assert from_tensors == from_dict
+    only_ungrouped = [(c, c + 1) for c in range(0, 40, 2)]      # ... and some are linked only to each other
+    ints = rng.integers(1, 3, len(ki)).tolist()                 # 1 or 2 links: ties everywhere
+    frac = rng.choice([0.5, 0.25, 1.5, 0.1], len(ki)).tolist()
+    cases = {
+        "ints": ints,
+        # reduced inter-haplotype links beside counts
+        "mixed": [v if rng.random() < 0.5 else v - v * w for v, w in zip(ints, frac)],
+        # --remove_concentrated_links scaling: integral floats (`*= 1.0`) and 0.0 among them
+        "scaled": [v * r for v, r in zip(ints, rng.choice([1.0, 0.0, 0.5, 2.0], len(ki)).tolist())],
+    }
+    for tag, vals in cases.items():
+        d = {(names[a], names[b]): 3 if tag == "ints" else 3.0 for a, b in only_ungrouped}
+        for a, b, v in zip(ki, kj, vals):
+            if a >= 40:                                         # (a < b) contigs 0..39 keep only the links above
+                d[(names[a], names[b])] = v
+        la = cluster.LinkArrays.from_dict(names, d)
+        assert [list(k) + [repr(v)] for k, v in la.to_dict().items()] == [list(k) + [repr(v)] for k, v in d.items()], tag
+        assert (la.is_float is None) == (tag == "ints"), tag
+        gid, ng = so.group_ids(names, groups)
+        got = so.ranked_lists(names, *so.ranked_group_links(la, gid, ng))
+        want = so.ranked_from_dict(d, groups)
+        assert _typed_ranking(got) == _typed_ranking(want), tag
+        assert all(names[a] not in want for a, _b in only_ungrouped)
+        if tag == "scaled":
+            assert any(v == 0.0 for lst in want.values() for _g, v in lst)
+            assert any(isinstance(v, float) and v == int(v) and v for lst in want.values() for _g, v in lst)
