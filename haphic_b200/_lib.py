@@ -76,6 +76,7 @@ _SIGNATURES = {
     "hh_links_agg_info": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "hh_links_fetch": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "hh_links_fetch_phased": (C.c_int, [_P, _P, C.c_double, _P, _P, _P, _P, C.POINTER(C.c_int64)]),
+    "hh_links_set_ul_pairs": (C.c_int, [_P, _P, _P, _P, C.c_int64]),
     "hh_links_fetch_ctg": (C.c_int, [_P, _P]),
     "hh_stats_create": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, C.c_int64, C.POINTER(_P)]),
     "hh_stats_rank": (C.c_int, [_P, _P, C.c_int32, C.POINTER(C.c_int64)]),
@@ -93,6 +94,7 @@ _SIGNATURES = {
     "hh_matrix_from_links": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int, C.c_int, C.POINTER(_P)]),
     "hh_links_linked_index_phased": (C.c_int, [_P, _P, C.c_int, _P, C.c_double, _P, C.POINTER(C.c_int32)]),
     "hh_matrix_from_links_phased": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int, C.c_int, _P, C.c_double, C.POINTER(_P)]),
+    "hh_matrix_from_links_ex": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int, C.c_int, _P, C.c_double, _P, _P, C.POINTER(_P)]),
     "hh_matrix_rank_sums": (C.c_int, [_P, C.c_int, _P]),
     "hh_matrix_from_csc": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "hh_matrix_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
@@ -136,6 +138,10 @@ _SIGNATURES = {
     "hh_bam_header_text": (C.c_int, [_P, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
     "hh_bam_next": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "hh_bam_close": (C.c_int, [_P]),
+    "hh_ul_open": (C.c_int, [C.c_char_p, C.c_int, C.c_int32, C.c_int64, C.c_int64, C.c_double, C.c_int64, C.POINTER(_P)]),
+    "hh_ul_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hh_ul_fetch": (C.c_int, [_P, _P, _P, _P]),
+    "hh_ul_close": (C.c_int, [_P]),
     "hh_pickle_links": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P]),
     "hh_pickle_links_mixed": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, _P, C.c_int64, _P, _P]),
     "hh_clm_from_records": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, C.c_int64, _P, _P, C.c_int]),

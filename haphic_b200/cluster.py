@@ -21,8 +21,13 @@ The reassignment statistics of every inflation (output_statistics) run on the de
 links: integer counts, ints and floats after a fractional phasing weight, and the host-edited dict of the
 ``--remove_allelic_links`` / ``--remove_concentrated_links`` runs.
 
-Not supported (raise, never silently degrade): ``--ul`` (ignored with a warning together with ``--correct_nrounds``, as
-in the reference).
+``--ul`` (ultra-long read alignments, a BAM) is read once by the native reader (hh_ul_open / hh_ul_info / hh_ul_fetch /
+hh_ul_close); haphic_b200/ul.py turns its link events into the reference's contig paths.  Their contigs form the
+whitelist; the HT and full links of adjacent path contigs are doubled when the device table is fetched
+(hh_links_set_ul_pairs), and the flank links between contigs of one path inside the device matrix kernels
+(hh_matrix_from_links_ex) -- or on the host dicts when allelic / concentrated-link removal edits them.  As in the reference,
+``--ul`` is ignored with a warning together with ``--correct_nrounds``.  The reference's per-entry stdout print of the
+doubled flank links is not reproduced.
 
 Reference line numbers below refer to scripts/HapHiC_cluster.py (v1.0.7).
 """
@@ -569,11 +574,12 @@ def _cut_index(sorted_pairs, limit, inclusive):
     return len(sorted_pairs)
 
 
-def device_matrix(table, names, frag_set, normalize_by_nlinks=False, add_self_loops=True, hap=None, phasing_weight=0.0):
+def device_matrix(table, names, frag_set, normalize_by_nlinks=False, add_self_loops=True, hap=None, phasing_weight=0.0, ul=None):
     """dict_to_matrix (310-373) on the device table: (LinkMatrix, frag_index_dict).  Linked fragments get their
     first-seen index on the GPU; kept-but-unlinked ones follow in the reference's set-iteration order (355-359).
     ``hap`` (haplotype per table fragment) builds it from the phasing-reduced dict (reduce_inter_hap_HiC_links): a
-    fragment whose links were all deleted joins the unlinked tail."""
+    fragment whose links were all deleted joins the unlinked tail.  ``ul`` = (ul_path, ul_parent) per table fragment
+    (ul.fragment_arrays) doubles the flank links of add_flank_and_full_links_based_on_ul first."""
     keep = np.fromiter((n in frag_set for n in names), dtype=np.uint8, count=len(names))
     index, n_linked = table.linked_index(keep, hap=hap, phasing_weight=phasing_weight, normalize_by_nlinks=normalize_by_nlinks)
     order = np.argsort(np.where(index >= 0, index, np.iinfo(np.int32).max), kind="stable")[:n_linked]
@@ -583,7 +589,7 @@ def device_matrix(table, names, frag_set, normalize_by_nlinks=False, add_self_lo
     ids = {n: i for i, n in enumerate(names)}
     tail = [ids[f] for f in frag_set - frags_in_dict]
     matrix = table.to_matrix(keep, tail, normalize_by_nlinks=normalize_by_nlinks, add_self_loops=add_self_loops, hap=hap,
-                             phasing_weight=phasing_weight)
+                             phasing_weight=phasing_weight, ul=ul)
     frag_index = {names[c]: int(index[c]) for c in order.tolist()}
     for k, c in enumerate(tail):
         frag_index[names[c]] = n_linked + k
@@ -1283,8 +1289,6 @@ def run(args, log_file=None):
     if args.correct_nrounds and args.ul:                   # 2774-2776
         args.ul = None
         logger.warning("Ultra-long data are not supported now when assembly correction is enabled")
-    if args.ul:
-        raise NotImplementedError("haphic_b200: --ul is not supported (out of the hot-path scope)")
     gfa_list = args.gfa.split(",") if args.gfa else []
     phasing = len(gfa_list) >= 2 and bool(args.phasing_weight)
     if phasing and not 0 <= args.phasing_weight <= 1:
@@ -1317,6 +1321,11 @@ def run(args, log_file=None):
         alignments, _nbroken = correct.run_correction(_context(), fa_dict, args, open_alignments(False),
                                                       lambda seq: count_RE_sites(seq, args.RE), read_depth_dict)
     ctg_read_depth_dict = read_depth_dict.copy()            # contig level; stat_fragments moves read_depth_dict to bins
+    path_list = []
+    if args.ul:                                             # 2813-2826
+        from . import ul
+        path_list = ul.parse_ul_alignments(args, logger)
+        whitelist.update(ul.whitelist(path_list))
     _, bin_set, bin_size, frag_len_dict, Nx_frag_set, RE_site_dict, split_ctg_set = stat_fragments(
         fa_dict, args.RE, read_depth_dict, whitelist, nchrs=args.nchrs, flank=args.flank, Nx=args.Nx, bin_size=args.bin_size)
     if alignments is None:
@@ -1327,7 +1336,7 @@ def run(args, log_file=None):
     # edited on the host, so they are built as the reference's Python objects.  Otherwise nothing on the host needs
     # them: the links stay arrays (LinkArrays), the pickles are written natively and no 10^7-entry dict is built.
     edits_dicts = bool(args.remove_allelic_links or args.remove_concentrated_links)
-    ctg_coord_dict, ctg_pair_to_frag, flank_link_dict = None, None, None
+    ctg_coord_dict, ctg_pair_to_frag, flank_link_dict, ul_present = None, None, None, None
     # pairs that reach max_read_pairs are always evaluated by the reference, whatever min_read_pairs says
     _COORD_SKIP[0] = 0 if (args.verbose or args.remove_concentrated_links) else min(int(args.min_read_pairs), int(args.max_read_pairs))
     if edits_dicts:
@@ -1343,6 +1352,8 @@ def run(args, log_file=None):
                 alignments, fa_dict, args, frag_len_dict, Nx_frag_set, pos_int_type, dist_int_type, build_clm=False)
             table = parse_alignments_for_ctgs.last_table
             clm_src = parse_alignments_for_ctgs.last_clm
+        if path_list:
+            ul.add_HT_links_based_on_ul(path_list, HT_link_dict, logger)
         output_pickle(HT_link_dict, "HT_link_dict", "HT_links.pkl")
         del HT_link_dict, clm_dict
     else:
@@ -1351,7 +1362,15 @@ def run(args, log_file=None):
             st = _stream_bins(alignments, fa_dict, args, bin_size, frag_len_dict, Nx_frag_set, split_ctg_set)
         else:
             st = _stream_contigs(alignments, fa_dict, args, frag_len_dict, Nx_frag_set)
+        if path_list:
+            # the HT and full links of adjacent path contigs are doubled as they are fetched (add_HT_links_based_on_ul and
+            # the full half of add_flank_and_full_links_based_on_ul): HT_links.pkl, full_links.pkl and the statistics
+            st["table"].set_ul_pairs(*ul.table_pairs(path_list, st["names"]))
         fetched = st["table"].fetch()
+        ul_present = None
+        if path_list and logger.isEnabledFor(logging.DEBUG):
+            ul_present = ul.present_keys(path_list, st["names"], fetched["key_i"], fetched["key_j"], fetched["ht"])
+            ul.add_HT_links_based_on_ul(path_list, ul_present[0], logger)        # debug lines only: doubled at the fetch
         full_link_dict = LinkArrays(st["names"], fetched["key_i"], fetched["key_j"], fetched["full"])
         logger.info("Writing {} to {}...".format("HT_link_dict", "HT_links.pkl"))
         full_link_dict.write_pickle("HT_links.pkl", ht=fetched["ht"])
@@ -1402,6 +1421,19 @@ def run(args, log_file=None):
         filtered_frags = remove_allelic_HiC_links(fa_dict, ctg_coord_dict, full_link_dict, args, flank_link_dict, filtered_frags,
                                                   ctg_pair_to_frag if split_ctg_set else None)
     del ctg_coord_dict
+    ul_frag = None
+    if path_list:                                           # 2921-2923
+        if flank_link_dict is not None:
+            ul.add_flank_and_full_links_based_on_ul(path_list, flank_link_dict, full_link_dict, bin_set, logger)
+        elif ul_present is not None:                        # debug lines only: the device doubles the links
+            ul.add_flank_and_full_links_based_on_ul(path_list, None, ul_present[1], bin_set, logger)
+        if not args.remove_allelic_links:                   # the matrix comes from the device table
+            if split_ctg_set:
+                frag_base = fragment_layout(fa_dict, bin_size, frag_len_dict, Nx_frag_set, split_ctg_set)[1]
+                parent = np.repeat(np.arange(len(frag_base) - 1, dtype=np.int32), np.diff(frag_base))
+            else:
+                parent = np.arange(len(names), dtype=np.int32)
+            ul_frag = ul.fragment_arrays(path_list, list(fa_dict), parent)
     hap = None
     if phasing:                                             # 2926-2928
         # the matrix comes from the device table unless allelic removal edited the host dict: the table's matrix kernels
@@ -1429,7 +1461,8 @@ def run(args, log_file=None):
         # dict_to_matrix on the device: first-seen indices from the table, unlinked fragments appended in
         # the reference's set-iteration order (355-359)
         link_matrix, frag_index_dict = device_matrix(table, names, filtered_frags, normalize_by_nlinks=args.normalize_by_nlinks,
-                                                     add_self_loops=True, hap=hap, phasing_weight=args.phasing_weight)
+                                                     add_self_loops=True, hap=hap, phasing_weight=args.phasing_weight,
+                                                     ul=ul_frag)
     table.close()
     matrix_time = time.time()
     logger.info("Hi-C linking matrix was constructed in {}s".format(matrix_time - start_time))

@@ -4,6 +4,7 @@
 //     the text is cut at line boundaries and parsed by a pool of threads, BGZF-compressed input is inflated
 //     block-parallel,
 //   * BAM reader (bam_generator, 1586-1593),
+//   * ultra-long read alignments for --ul (parse_ul_alignments, 1763-1869),
 //   * paired_links.clm from the record stream (update_clm_dict 395-401 + output_clm 376-392), threaded.
 // Pure C++ (no CUDA); part of libhaphic_b200.so, declared in include/haphic_b200.h.
 #include <stdint.h>
@@ -680,8 +681,7 @@ struct hh_bam_reader {
 };
 
 // make sure `need` decompressed bytes are available at raw_pos; returns 0 ok, 1 clean EOF (nothing left), -1 error
-static int bam_need(hh_bam_reader* rd, size_t need) {
-    hh_bgzf* r = &rd->z;
+static int bam_need(hh_bgzf* r, size_t need) {
     while (r->raw_len - r->raw_pos < need) {
         const int rc = bgzf_fill(r, 32u << 20);
         if (rc < 0) return -1;
@@ -716,11 +716,11 @@ extern "C" int hh_bam_open(const char* path, const char* names_blob, int32_t n_n
         delete r;
         return HH_ERR_ARG;
     };
-    if (bam_need(r, 12) != 0) return fail(nullptr);
+    if (bam_need(&r->z, 12) != 0) return fail(nullptr);
     const uint8_t* p = r->z.raw.data() + r->z.raw_pos;
     if (memcmp(p, "BAM\1", 4) != 0) return fail("hh_bam_open: not a BAM file");
     const size_t l_text = le32(p + 4);
-    if (bam_need(r, 12 + l_text) != 0) return fail(nullptr);
+    if (bam_need(&r->z, 12 + l_text) != 0) return fail(nullptr);
     p = r->z.raw.data() + r->z.raw_pos;
     r->header_text.assign(reinterpret_cast<const char*>(p + 8), l_text);
     while (!r->header_text.empty() && r->header_text.back() == '\0') r->header_text.pop_back();
@@ -730,9 +730,9 @@ extern "C" int hh_bam_open(const char* path, const char* names_blob, int32_t n_n
     ids.build(names_blob, n_names);
     r->ref_to_id.assign((size_t)(n_ref > 0 ? n_ref : 0), -1);
     for (int32_t k = 0; k < n_ref; ++k) {
-        if (bam_need(r, 4) != 0) return fail("hh_bam_open: truncated BAM header");
+        if (bam_need(&r->z, 4) != 0) return fail("hh_bam_open: truncated BAM header");
         const size_t l_name = le32(r->z.raw.data() + r->z.raw_pos);
-        if (bam_need(r, 8 + l_name) != 0) return fail("hh_bam_open: truncated BAM header");
+        if (bam_need(&r->z, 8 + l_name) != 0) return fail("hh_bam_open: truncated BAM header");
         const char* nm = reinterpret_cast<const char*>(r->z.raw.data() + r->z.raw_pos + 4);
         r->ref_to_id[(size_t)k] = ids.find(nm, l_name ? l_name - 1 : 0);
         r->z.raw_pos += 8 + l_name;
@@ -760,7 +760,7 @@ extern "C" int hh_bam_next(hh_bam_reader* r, int32_t* rec, int64_t max_records, 
     *n_out = 0;
     const int32_t n_ref = (int32_t)r->ref_to_id.size();
     while (n < max_records) {
-        int rc = bam_need(r, 4);
+        int rc = bam_need(&r->z, 4);
         if (rc == 1) break;
         if (rc < 0) return HH_ERR_ARG;
         const size_t bs = le32(r->z.raw.data() + r->z.raw_pos);
@@ -768,7 +768,7 @@ extern "C" int hh_bam_next(hh_bam_reader* r, int32_t* rec, int64_t max_records, 
             hh_set_error("hh_bam_next: corrupt BAM record (block_size %zu)", bs);
             return HH_ERR_ARG;
         }
-        rc = bam_need(r, 4 + bs);
+        rc = bam_need(&r->z, 4 + bs);
         if (rc != 0) {
             if (rc == 1) hh_set_error("hh_bam_next: truncated BAM record");
             return HH_ERR_ARG;
@@ -795,6 +795,283 @@ extern "C" int hh_bam_next(hh_bam_reader* r, int32_t* rec, int64_t max_records, 
 extern "C" int hh_bam_close(hh_bam_reader* r) {
     if (!r) return HH_OK;
     if (r->z.f) fclose(r->z.f);
+    delete r;
+    return HH_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Ultra-long read alignments (parse_ul_alignments, 1763-1869): one pass over the BAM with the htslib filter
+// `!flag.unmap`, the MAPQ / length / end-distance filters, the primary / supplementary state machine and the best
+// supplementary by AS.  What is kept is the header's references and one event per accepted (primary, supplementary)
+// pair: the semi-contigs (2 * ref + 0 for `_H`, 1 for `_T`) of the inter-contig edge, the primary's reference and the
+// supplementary's reference -- the three add_edge calls of parse_supplementary_aln_list, in file order.
+// ---------------------------------------------------------------------------------------------
+struct hh_ul_reader {
+    std::string names;                // reference names, NUL-terminated, header order
+    std::vector<int64_t> ref_len;
+    std::vector<int32_t> events;      // [n][4]
+    int64_t n_records = 0;
+};
+
+namespace {
+struct ul_aln {
+    int32_t ref;
+    bool reverse;
+    int64_t qs, qe;                   // query termini of get_query_alignment_termini
+    bool has_as;
+    int64_t as;
+};
+
+enum { CIG_M = 0, CIG_I = 1, CIG_D = 2, CIG_N = 3, CIG_S = 4, CIG_H = 5, CIG_EQ = 7, CIG_X = 8 };
+
+// integer value of the aux tag `tag` (types c C s S i I); false when absent or not an integer
+bool ul_aux_int(const uint8_t* p, const uint8_t* end, const char* tag, int64_t* v) {
+    while (p + 3 <= end) {
+        const bool hit = p[0] == (uint8_t)tag[0] && p[1] == (uint8_t)tag[1];
+        const char t = (char)p[2];
+        p += 3;
+        size_t sz = 0;
+        switch (t) {
+            case 'A': case 'c': case 'C': sz = 1; break;
+            case 's': case 'S': sz = 2; break;
+            case 'i': case 'I': case 'f': sz = 4; break;
+            case 'd': sz = 8; break;
+            case 'Z': case 'H': {
+                const uint8_t* q = p;
+                while (q < end && *q) ++q;
+                sz = (size_t)(q - p) + 1;
+                break;
+            }
+            case 'B': {
+                if (p + 5 > end) return false;
+                const char sub = (char)p[0];
+                const size_t cnt = le32(p + 1);
+                const size_t es = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : 4;
+                sz = 5 + cnt * es;
+                break;
+            }
+            default: return false;
+        }
+        if (p + sz > end) return false;
+        if (hit) {
+            switch (t) {
+                case 'c': *v = (int8_t)p[0]; return true;
+                case 'C': *v = p[0]; return true;
+                case 's': *v = (int16_t)le16(p); return true;
+                case 'S': *v = le16(p); return true;
+                case 'i': *v = (int32_t)le32(p); return true;
+                case 'I': *v = le32(p); return true;
+                default: return false;
+            }
+        }
+        p += sz;
+    }
+    return false;
+}
+}  // namespace
+
+extern "C" int hh_ul_open(const char* path, int threads, int32_t min_mapq, int64_t min_alignment_length, int64_t max_distance_to_end,
+                          double max_overlap_ratio, int64_t max_gap_len, hh_ul_reader** out) {
+    if (!path || !out) {
+        hh_set_error("hh_ul_open: bad argument");
+        return HH_ERR_ARG;
+    }
+    *out = nullptr;
+    hh_bgzf z;
+    z.f = fopen(path, "rb");
+    if (!z.f) {
+        hh_set_error("hh_ul_open: cannot open %s", path);
+        return HH_ERR_ARG;
+    }
+    z.threads = hh_io_threads(threads);
+    hh_ul_reader* r = new hh_ul_reader();
+    const int rc = [&]() -> int {
+        if (bam_need(&z, 12) != 0) {
+            hh_set_error("hh_ul_open: %s is empty or not a BAM file", path);
+            return HH_ERR_ARG;
+        }
+        const uint8_t* p = z.raw.data() + z.raw_pos;
+        if (memcmp(p, "BAM\1", 4) != 0) {
+            hh_set_error("hh_ul_open: %s is not a BAM file", path);
+            return HH_ERR_ARG;
+        }
+        const size_t l_text = le32(p + 4);
+        if (bam_need(&z, 12 + l_text) != 0) {
+            hh_set_error("hh_ul_open: truncated BAM header in %s", path);
+            return HH_ERR_ARG;
+        }
+        const int32_t n_ref = (int32_t)le32(z.raw.data() + z.raw_pos + 8 + l_text);
+        z.raw_pos += 12 + l_text;
+        for (int32_t k = 0; k < n_ref; ++k) {
+            if (bam_need(&z, 4) != 0) {
+                hh_set_error("hh_ul_open: truncated BAM header in %s", path);
+                return HH_ERR_ARG;
+            }
+            const size_t l_name = le32(z.raw.data() + z.raw_pos);
+            if (l_name == 0 || bam_need(&z, 8 + l_name) != 0) {
+                hh_set_error("hh_ul_open: truncated BAM header");
+                return HH_ERR_ARG;
+            }
+            const char* nm = reinterpret_cast<const char*>(z.raw.data() + z.raw_pos + 4);
+            r->names.append(nm, strnlen(nm, l_name));
+            r->names.push_back('\0');
+            r->ref_len.push_back((int32_t)le32(z.raw.data() + z.raw_pos + 4 + l_name));
+            z.raw_pos += 8 + l_name;
+        }
+        bool have_primary = false;
+        ul_aln prim{};
+        std::string prim_name;
+        std::vector<ul_aln> supp;
+        auto emit = [&]() -> int {
+            // the best supplementary: stable sort by AS, descending (only when there is a choice)
+            size_t best = 0;
+            if (supp.size() > 1) {
+                for (const ul_aln& s : supp)
+                    if (!s.has_as) {
+                        hh_set_error("hh_ul: supplementary alignment of %s without an integer AS tag", prim_name.c_str());
+                        return HH_ERR_ARG;
+                    }
+                for (size_t k = 1; k < supp.size(); ++k)
+                    if (supp[k].as > supp[best].as) best = k;
+            }
+            const ul_aln& s = supp[best];
+            // the two semi-contig pairs in read order (stable: the primary first on a tie)
+            const ul_aln& a = (s.qs < prim.qs) ? s : prim;
+            const ul_aln& b = (s.qs < prim.qs) ? prim : s;
+            const int32_t ev[4] = {2 * a.ref + (a.reverse ? 0 : 1), 2 * b.ref + (b.reverse ? 1 : 0), prim.ref, s.ref};
+            r->events.insert(r->events.end(), ev, ev + 4);
+            return HH_OK;
+        };
+        for (;;) {
+            int need = bam_need(&z, 4);
+            if (need == 1) break;
+            if (need < 0) return HH_ERR_ARG;                      // bgzf_fill / bam_need set the message
+            const size_t bs = le32(z.raw.data() + z.raw_pos);
+            if (bs < 32 || bam_need(&z, 4 + bs) != 0) {
+                hh_set_error("hh_ul: corrupt or truncated BAM record");
+                return HH_ERR_ARG;
+            }
+            const uint8_t* p = z.raw.data() + z.raw_pos + 4;
+            const uint8_t* end = p + bs;
+            z.raw_pos += 4 + bs;
+            r->n_records++;
+            const int32_t refid = (int32_t)le32(p), pos = (int32_t)le32(p + 4);
+            const uint8_t l_read_name = p[8], mapq = p[9];
+            const uint16_t n_cigar = le16(p + 12), flag = le16(p + 14);
+            const int32_t l_seq = (int32_t)le32(p + 16);
+            if (flag & 0x4) continue;                                 // filter=!flag.unmap
+            const uint8_t* name = p + 32;
+            const uint8_t* cig = name + l_read_name;
+            const uint8_t* aux = cig + 4 * (size_t)n_cigar + ((size_t)l_seq + 1) / 2 + (size_t)l_seq;
+            if (aux > end || refid < 0 || refid >= n_ref) {
+                hh_set_error("hh_ul: corrupt BAM record (mapped record without a reference, or fields past its end)");
+                return HH_ERR_ARG;
+            }
+            if (n_cigar == 0) {
+                hh_set_error("hh_ul: mapped record without a CIGAR (reference_length undefined)");
+                return HH_ERR_ARG;
+            }
+            int64_t ref_span = 0, read_len = 0, qs = 0, qe = 0, qe_noseq = 0;
+            bool lead = true;
+            for (uint16_t k = 0; k < n_cigar; ++k) {
+                const uint32_t c = le32(cig + 4 * k);
+                const uint32_t op = c & 15, ln = c >> 4;
+                if (op == CIG_M || op == CIG_D || op == CIG_N || op == CIG_EQ || op == CIG_X) ref_span += ln;
+                if (op == CIG_M || op == CIG_I || op == CIG_S || op == CIG_EQ || op == CIG_X || op == CIG_H) read_len += ln;
+                // pysam query_alignment_start: soft clips before the first aligned operation (hard clips skipped)
+                if (lead) {
+                    if (op == CIG_S) qs += ln;
+                    else if (op != CIG_H) lead = false;
+                }
+                // pysam query_alignment_end without SEQ: M / I / = / X lengths plus a soft clip met while the sum is 0
+                if (op == CIG_M || op == CIG_I || op == CIG_EQ || op == CIG_X || (op == CIG_S && qe_noseq == 0)) qe_noseq += ln;
+            }
+            if (l_seq == 0) {
+                qe = qe_noseq;
+            } else {
+                // with SEQ: l_qseq less the trailing soft clips (hard clips skipped; the first operation is never examined)
+                qe = l_seq;
+                for (int k = (int)n_cigar - 1; k >= 1; --k) {
+                    const uint32_t c = le32(cig + 4 * k);
+                    const uint32_t op = c & 15;
+                    if (op == CIG_S) qe -= c >> 4;
+                    else if (op != CIG_H) break;
+                }
+            }
+            if (mapq < min_mapq || ref_span < min_alignment_length) continue;
+            if (pos > max_distance_to_end && r->ref_len[(size_t)refid] - (pos + ref_span) > max_distance_to_end) continue;
+            ul_aln a;
+            a.ref = refid;
+            a.reverse = (flag & 0x10) != 0;
+            if (!a.reverse) {
+                const uint32_t c0 = le32(cig);
+                const int64_t hc = ((c0 & 15) == CIG_H) ? (int64_t)(c0 >> 4) : 0;
+                a.qs = qs + hc;
+                a.qe = qe + hc;
+            } else {
+                const uint32_t cl = le32(cig + 4 * ((size_t)n_cigar - 1));
+                const int64_t hc = ((cl & 15) == CIG_H) ? (int64_t)(cl >> 4) : 0;
+                a.qs = read_len - qe + hc;
+                a.qe = read_len - qs + hc;
+            }
+            a.has_as = ul_aux_int(aux, end, "AS", &a.as);
+            const char* nm = reinterpret_cast<const char*>(name);
+            const size_t nm_len = strnlen(nm, l_read_name);
+            if (flag == 0 || flag == 16) {
+                if (!supp.empty() && emit() != HH_OK) return HH_ERR_ARG;
+                prim = a;
+                prim_name.assign(nm, nm_len);
+                have_primary = true;
+                supp.clear();
+            } else if ((flag & 0x800) && have_primary && prim_name.size() == nm_len && memcmp(prim_name.data(), nm, nm_len) == 0 &&
+                       refid != prim.ref) {
+                // query intervals closed(start + 1, end) of the primary and the supplementary
+                const int64_t lo = std::max(prim.qs, a.qs) + 1, hi = std::min(prim.qe, a.qe);
+                if (lo <= hi) {
+                    const double ratio = (double)(hi - lo + 1) / (double)std::min(prim.qe - prim.qs, a.qe - a.qs);
+                    if (ratio > max_overlap_ratio) continue;
+                } else if (lo - hi + 1 > max_gap_len) {
+                    continue;                                     // the open gap between them, measured as if closed
+                }
+                supp.push_back(a);
+            }
+        }
+        if (!supp.empty() && emit() != HH_OK) return HH_ERR_ARG;
+        return HH_OK;
+    }();
+    fclose(z.f);
+    if (rc != HH_OK) {
+        delete r;
+        return rc;
+    }
+    *out = r;
+    return HH_OK;
+}
+
+extern "C" int hh_ul_info(hh_ul_reader* r, int32_t* n_ref, int64_t* names_bytes, int64_t* n_events, int64_t* n_records) {
+    if (!r) {
+        hh_set_error("hh_ul_info: NULL handle");
+        return HH_ERR_ARG;
+    }
+    if (n_ref) *n_ref = (int32_t)r->ref_len.size();
+    if (names_bytes) *names_bytes = (int64_t)r->names.size();
+    if (n_events) *n_events = (int64_t)(r->events.size() / 4);
+    if (n_records) *n_records = r->n_records;
+    return HH_OK;
+}
+
+extern "C" int hh_ul_fetch(hh_ul_reader* r, char* names, int64_t* ref_len, int32_t* events) {
+    if (!r) {
+        hh_set_error("hh_ul_fetch: NULL handle");
+        return HH_ERR_ARG;
+    }
+    if (names && !r->names.empty()) memcpy(names, r->names.data(), r->names.size());
+    if (ref_len && !r->ref_len.empty()) memcpy(ref_len, r->ref_len.data(), r->ref_len.size() * sizeof(int64_t));
+    if (events && !r->events.empty()) memcpy(events, r->events.data(), r->events.size() * sizeof(int32_t));
+    return HH_OK;
+}
+
+extern "C" int hh_ul_close(hh_ul_reader* r) {
     delete r;
     return HH_OK;
 }

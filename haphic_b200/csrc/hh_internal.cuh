@@ -18,13 +18,16 @@ struct hh_matrix {
 enum { HH_E_I, HH_E_J, HH_E_FULL, HH_E_FLANK, HH_E_FIRST_FULL, HH_E_FIRST_FLANK, HH_E_HT, HH_E_TH, HH_E_TT, HH_E_WORDS };
 
 // How the matrix sees one entry of the compact link table: the flank count, or
-// links / (tot_i * tot_j) ** 0.5 in fp64 with normalize (normalize_by_nlinks, 718-724), then -- when hap != NULL and the
-// two ends lie on different haplotypes -- x - x * w with two roundings (reduce_inter_hap_HiC_links, 695-707).  Returns
-// false when the entry is not in the (reduced) flank_link_dict: no flank link, or reduced to exactly 0.  hh_k_touch
-// and hh_k_mat_scatter both decide through this one function, so pattern, values and first-seen indices
-// cannot disagree.
+// links / (tot_i * tot_j) ** 0.5 in fp64 with normalize (normalize_by_nlinks, 718-724), then x 2 when ul_path != NULL and
+// the two ends lie on two different contigs (ul_parent) of one ultra-long-read path (add_flank_and_full_links_based_on_ul,
+// 1936-1985), then -- when hap != NULL and the two ends lie on different haplotypes -- x - x * w with two roundings
+// (reduce_inter_hap_HiC_links, 695-707).  Returns false when the entry is not in the (reduced) flank_link_dict: no flank
+// link, or reduced to exactly 0.  hh_k_touch and hh_k_mat_scatter both decide through this one function, so pattern,
+// values and first-seen indices cannot disagree; doubling never makes a value 0, so the index pass may leave ul_path NULL.
 __device__ __forceinline__ bool hh_flank_value(const uint32_t* __restrict__ p, const unsigned long long* __restrict__ ctg_tot,
-                                               int normalize, const int32_t* __restrict__ hap, double w, double* x_out) {
+                                               int normalize, const int32_t* __restrict__ hap, double w,
+                                               const int32_t* __restrict__ ul_path, const int32_t* __restrict__ ul_parent,
+                                               double* x_out) {
     if (p[HH_E_FLANK] == 0) return false;
     double x;
     if (normalize) {
@@ -32,6 +35,10 @@ __device__ __forceinline__ bool hh_flank_value(const uint32_t* __restrict__ p, c
         x = (double)p[HH_E_FLANK] / pow((double)prod, 0.5);
     } else {
         x = (double)p[HH_E_FLANK];
+    }
+    if (ul_path != nullptr) {
+        const int32_t pi = ul_path[p[HH_E_I]];
+        if (pi >= 0 && pi == ul_path[p[HH_E_J]] && ul_parent[p[HH_E_I]] != ul_parent[p[HH_E_J]]) x *= 2.0;
     }
     if (hap != nullptr && hap[p[HH_E_I]] != hap[p[HH_E_J]]) x = __dsub_rn(x, __dmul_rn(x, w));
     if (x == 0.0) return false;

@@ -91,6 +91,10 @@ struct hh_links {
     double ix_w;
     std::vector<uint8_t> ix_keep;
     std::vector<int32_t> ix_hap;     // empty: unphased
+    // contig pairs joined by ultra-long reads (hh_links_set_ul_pairs): keys (i << 32 | j) ascending, the HT slot of each
+    unsigned long long* d_ul_key = nullptr;
+    int32_t* d_ul_slot = nullptr;
+    int64_t n_ul = 0;
 };
 
 __device__ __forceinline__ uint64_t hh_mix64(uint64_t k) {
@@ -1213,7 +1217,7 @@ hh_k_touch(const uint32_t* __restrict__ compact, int64_t nnz, const uint8_t* __r
         const uint32_t i = p[HH_E_I], j = p[HH_E_J];
         if (!keep[i] || !keep[j]) continue;            // 329-330
         double x;
-        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;   // not in flank_link_dict
+        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, nullptr, nullptr, &x)) continue;   // not in flank_link_dict
         const unsigned long long t = (unsigned long long)p[HH_E_FIRST_FLANK] * 2ull;
         // touch values only fall, so a value read from L2 that is already below t makes the atomic a no-op; most are
         if (t < __ldcg(touch + i)) atomicMin(touch + i, t);
@@ -1869,7 +1873,24 @@ extern "C" int hh_links_finish(hh_links* lk, hh_links_info* info) {
 }
 
 // AoS compact entries -> the 7 output arrays (SoA), so each goes to the host with one plain copy
-__global__ void hh_k_links_split(const uint32_t* __restrict__ compact, int64_t nnz, uint32_t* __restrict__ soa, int64_t ht_off) {
+// HT slot of the ultra-long-read pair (i, j), -1 when the pair is not on the list (binary search of the sorted keys)
+__device__ __forceinline__ int hh_ul_slot(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ slot, int64_t n,
+                                          uint32_t i, uint32_t j) {
+    const unsigned long long key = ((unsigned long long)i << 32) | j;
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (keys[mid] < key) lo = mid + 1;
+        else hi = mid;
+    }
+    return (lo < n && keys[lo] == key) ? slot[lo] : -1;
+}
+
+// ul_key / ul_slot / n_ul: the full count and one HT slot of the listed pairs are doubled (HH from the stored counts);
+// *overflow is set when a doubled count does not fit 32 bits
+__global__ void hh_k_links_split(const uint32_t* __restrict__ compact, int64_t nnz, uint32_t* __restrict__ soa, int64_t ht_off,
+                                 const unsigned long long* __restrict__ ul_key, const int32_t* __restrict__ ul_slot, int64_t n_ul,
+                                 int* __restrict__ overflow) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
         const uint32_t* p = compact + e * HH_E_WORDS;
@@ -1880,6 +1901,17 @@ __global__ void hh_k_links_split(const uint32_t* __restrict__ compact, int64_t n
         h.z = p[HH_E_TH];
         h.w = p[HH_E_TT];
         h.x = p[HH_E_FULL] - p[HH_E_HT] - p[HH_E_TH] - p[HH_E_TT];          // HH = full - HT - TH - TT
+        const int s = n_ul ? hh_ul_slot(ul_key, ul_slot, n_ul, p[HH_E_I], p[HH_E_J]) : -1;
+        if (s >= 0) {
+            // selects rather than h[s]: a runtime index would put the four words in local memory
+            const uint32_t hs = s == 0 ? h.x : s == 1 ? h.y : s == 2 ? h.z : h.w;
+            if (p[HH_E_FULL] > 0x7FFFFFFFu || hs > 0x7FFFFFFFu) atomicExch(overflow, 1);
+            soa[HH_E_FULL * nnz + e] = p[HH_E_FULL] * 2u;
+            h.x = s == 0 ? h.x * 2u : h.x;
+            h.y = s == 1 ? h.y * 2u : h.y;
+            h.z = s == 2 ? h.z * 2u : h.z;
+            h.w = s == 3 ? h.w * 2u : h.w;
+        }
         reinterpret_cast<uint4*>(soa + ht_off)[e] = h;
     }
 }
@@ -2045,13 +2077,18 @@ extern "C" int hh_links_fetch(hh_links* lk, int32_t* key_i, int32_t* key_j, uint
         uint32_t* base = d_soa;
         const int64_t ht_off = (6 * nnz + 3) & ~3ll;      // the 4-wide HT block is written with 16-byte stores
         const int grid = links_grid(ctx, nnz);
-        HH_LAUNCH(ctx, hh_k_links_split, grid, 256, 0, lk->d_compact, nnz, base, ht_off);
+        int* d_err = reinterpret_cast<int*>(ctx->d_scratch + 10);
+        HH_CUDA(cudaMemsetAsync(d_err, 0, sizeof(int), ctx->stream));
+        HH_LAUNCH(ctx, hh_k_links_split, grid, 256, 0, lk->d_compact, nnz, base, ht_off, lk->d_ul_key, lk->d_ul_slot, lk->n_ul, d_err);
         void* dst[6] = {key_i, key_j, full, flank, first_full, first_flank};
         for (int k = 0; k < 6; ++k)
             if (dst[k])
                 HH_CUDA(cudaMemcpyAsync(dst[k], base + (size_t)k * nnz, (size_t)nnz * 4, cudaMemcpyDeviceToHost, ctx->stream));
         if (ht) HH_CUDA(cudaMemcpyAsync(ht, base + ht_off, (size_t)nnz * 16, cudaMemcpyDeviceToHost, ctx->stream));
+        HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 10, d_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaStreamSynchronize(ctx->stream));
+        HH_REQUIRE(*reinterpret_cast<int*>(ctx->h_scratch + 10) == 0, HH_ERR_UNSUPPORTED,
+                   "hh_links_fetch: an ultra-long-read doubled link count exceeds 2^32 - 1");
         return HH_OK;
     }();
     hh_dfree(d_soa);
@@ -2086,12 +2123,16 @@ hh_k_phased_mark(const uint32_t* __restrict__ compact, int64_t nnz, const int32_
 // the kept entries -> key_i, key_j, values, is_float (SoA: int32 | int32 | fp64 | uint8 blocks of n)
 __global__ void __launch_bounds__(256)
 hh_k_phased_split(const uint32_t* __restrict__ kept, int64_t n, const int32_t* __restrict__ hap, double w, int32_t* __restrict__ ki,
-                  int32_t* __restrict__ kj, double* __restrict__ val, uint8_t* __restrict__ flt) {
+                  int32_t* __restrict__ kj, double* __restrict__ val, uint8_t* __restrict__ flt,
+                  const unsigned long long* __restrict__ ul_key, const int32_t* __restrict__ ul_slot, int64_t n_ul) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
         const uint32_t* p = kept + e * HH_E_WORDS;
         bool f;
-        val[e] = hh_full_value(p, hap, w, &f);
+        // an ultra-long-read pair counts twice before the reduction (1936-1985 runs before 2926-2928); 2 x - 2 x w is
+        // exactly 2 (x - x w), so the value is the reduced count doubled and zero exactly when that is
+        const bool ul = n_ul && hh_ul_slot(ul_key, ul_slot, n_ul, p[HH_E_I], p[HH_E_J]) >= 0;
+        val[e] = (ul ? 2.0 : 1.0) * hh_full_value(p, hap, w, &f);
         ki[e] = (int32_t)p[HH_E_I];
         kj[e] = (int32_t)p[HH_E_J];
         flt[e] = f;
@@ -2133,7 +2174,8 @@ extern "C" int hh_links_fetch_phased(hh_links* lk, const int32_t* hap, double w,
         int32_t* ki = reinterpret_cast<int32_t*>(d_soa);
         double* val = reinterpret_cast<double*>(d_soa + (size_t)n * 8);
         uint8_t* flt = d_soa + (size_t)n * 16;
-        HH_LAUNCH(ctx, hh_k_phased_split, links_grid(ctx, n), 256, 0, d_kept, n, d_hap, w, ki, ki + n, val, flt);
+        HH_LAUNCH(ctx, hh_k_phased_split, links_grid(ctx, n), 256, 0, d_kept, n, d_hap, w, ki, ki + n, val, flt, lk->d_ul_key,
+                  lk->d_ul_slot, lk->n_ul);
         HH_CUDA(cudaMemcpyAsync(key_i, ki, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaMemcpyAsync(key_j, ki + n, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaMemcpyAsync(values, val, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2147,6 +2189,42 @@ extern "C" int hh_links_fetch_phased(hh_links* lk, const int32_t* hap, double w,
     hh_dfree(d_soa);
     hh_dfree(d_n);
     return rc;
+}
+
+extern "C" int hh_links_set_ul_pairs(hh_links* lk, const int32_t* key_i, const int32_t* key_j, const int32_t* ht_slot, int64_t n_pairs) {
+    HH_REQUIRE(lk && n_pairs >= 0 && (n_pairs == 0 || (key_i && key_j && ht_slot)), HH_ERR_ARG, "hh_links_set_ul_pairs: bad argument");
+    hh_scope _scope(lk->ctx);
+    hh_ctx* ctx = lk->ctx;
+    HH_CUDA(cudaSetDevice(ctx->device));
+    std::vector<std::pair<unsigned long long, int32_t>> pairs((size_t)n_pairs);
+    for (int64_t k = 0; k < n_pairs; ++k) {
+        HH_REQUIRE(key_i[k] >= 0 && key_i[k] < lk->n_ctg && key_j[k] >= 0 && key_j[k] < lk->n_ctg && key_i[k] != key_j[k] &&
+                       ht_slot[k] >= 0 && ht_slot[k] < 4,
+                   HH_ERR_ARG, "hh_links_set_ul_pairs: pair %lld is out of range", (long long)k);
+        pairs[(size_t)k] = {((unsigned long long)key_i[k] << 32) | (uint32_t)key_j[k], ht_slot[k]};
+    }
+    std::sort(pairs.begin(), pairs.end());
+    for (size_t k = 1; k < pairs.size(); ++k)
+        HH_REQUIRE(pairs[k].first != pairs[k - 1].first, HH_ERR_ARG, "hh_links_set_ul_pairs: a contig pair is listed twice");
+    hh_dfree(lk->d_ul_key);
+    hh_dfree(lk->d_ul_slot);
+    lk->d_ul_key = nullptr;
+    lk->d_ul_slot = nullptr;
+    lk->n_ul = 0;
+    if (n_pairs == 0) return HH_OK;
+    std::vector<unsigned long long> keys((size_t)n_pairs);
+    std::vector<int32_t> slots((size_t)n_pairs);
+    for (size_t k = 0; k < pairs.size(); ++k) {
+        keys[k] = pairs[k].first;
+        slots[k] = pairs[k].second;
+    }
+    HH_CHECK(hh_dmalloc(&lk->d_ul_key, (size_t)n_pairs));
+    HH_CHECK(hh_dmalloc(&lk->d_ul_slot, (size_t)n_pairs));
+    HH_CUDA(cudaMemcpyAsync(lk->d_ul_key, keys.data(), keys.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, ctx->stream));
+    HH_CUDA(cudaMemcpyAsync(lk->d_ul_slot, slots.data(), slots.size() * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    HH_CUDA(cudaStreamSynchronize(ctx->stream));
+    lk->n_ul = n_pairs;
+    return HH_OK;
 }
 
 extern "C" int hh_links_fetch_ctg(hh_links* lk, int64_t* ctg_links) {
@@ -2311,6 +2389,8 @@ extern "C" int hh_links_destroy(hh_links* lk) {
     hh_dfree(lk->d_keep);
     hh_dfree(lk->d_hap);
     hh_dfree(lk->d_deg);
+    hh_dfree(lk->d_ul_key);
+    hh_dfree(lk->d_ul_slot);
     links_free_partsets(lk);
     delete lk;
     return HH_OK;

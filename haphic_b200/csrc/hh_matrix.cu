@@ -53,7 +53,8 @@ __global__ void hh_k_mat_self_loops(int n, const int64_t* __restrict__ colptr, i
 // every passing entry to its two columns; the order of rows inside a column is left unspecified
 __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
                                  const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
-                                 double w, const int64_t* __restrict__ colptr, int* __restrict__ cursor,
+                                 double w, const int32_t* __restrict__ ul_path, const int32_t* __restrict__ ul_parent,
+                                 const int64_t* __restrict__ colptr, int* __restrict__ cursor,
                                  int32_t* __restrict__ row, float* __restrict__ val) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
@@ -62,7 +63,7 @@ __global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t n
         const int ii = index[p[HH_E_I]], jj = index[p[HH_E_J]];
         if (ii < 0 || jj < 0) continue;                 // 329-330
         double x;
-        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, &x)) continue;
+        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, ul_path, ul_parent, &x)) continue;
         const float v = (float)x;                      // coo_matrix(dtype=float32) (368)
         int64_t q = colptr[jj] + atomicAdd(cursor + jj, 1);    // (row ii, col jj)
         row[q] = ii;
@@ -98,9 +99,16 @@ extern "C" int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int
 extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
                                            int normalize_by_nlinks, int add_self_loops, const int32_t* hap, double w,
                                            hh_matrix** out) {
+    return hh_matrix_from_links_ex(lk, keep, tail, n_tail, normalize_by_nlinks, add_self_loops, hap, w, nullptr, nullptr, out);
+}
+
+extern "C" int hh_matrix_from_links_ex(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail, int normalize_by_nlinks,
+                                       int add_self_loops, const int32_t* hap, double w, const int32_t* ul_path,
+                                       const int32_t* ul_parent, hh_matrix** out) {
     HH_REQUIRE(lk && keep && out, HH_ERR_ARG, "hh_matrix_from_links: NULL argument");
     hh_scope _scope(hh_links_ctx(lk));
     HH_REQUIRE(n_tail >= 0 && (tail || n_tail == 0), HH_ERR_ARG, "hh_matrix_from_links: bad tail");
+    HH_REQUIRE(!ul_path == !ul_parent, HH_ERR_ARG, "hh_matrix_from_links_ex: give both ul_path and ul_parent, or neither");
     HH_REQUIRE(hh_links_finished(lk), HH_ERR_STATE, "hh_matrix_from_links: call hh_links_finish first");
     *out = nullptr;
     hh_ctx* ctx = hh_links_ctx(lk);
@@ -124,6 +132,7 @@ extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, co
     const int64_t nnz = 2 * n_pass + (int64_t)sl * n;      // known before any sync: the matrix is allocated up front
     int* d_err = reinterpret_cast<int*>(ctx->d_scratch + 10);
     int32_t* d_tail = nullptr;
+    int32_t* d_ul = nullptr;
     int* d_cnt = nullptr;
     hh_matrix* m = nullptr;
     int rc = [&]() -> int {
@@ -148,12 +157,17 @@ extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, co
         if (sl) HH_LAUNCH(ctx, hh_k_mat_self_loops, (n + 255) / 256, 256, 0, n, m->d_colptr, m->d_row, m->d_val);
         int64_t nnz_c = 0;
         const uint32_t* compact = hh_links_compact(lk, &nnz_c);
+        if (ul_path && n_pass) {
+            HH_CHECK(hh_dmalloc(&d_ul, (size_t)n_ctg * 2));
+            HH_CUDA(cudaMemcpyAsync(d_ul, ul_path, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+            HH_CUDA(cudaMemcpyAsync(d_ul + n_ctg, ul_parent, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+        }
         if (n_pass) {
             int gridc = 0;
             HH_CHECK(hh_resident_grid(ctx, hh_k_mat_scatter, 256, 0, &gridc));
             gridc = (int)std::min<int64_t>((nnz_c + 255) / 256, gridc);
             HH_LAUNCH(ctx, hh_k_mat_scatter, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks, d_hap,
-                      w, m->d_colptr, d_cursor, m->d_row, m->d_val);
+                      w, d_ul, d_ul ? d_ul + n_ctg : nullptr, m->d_colptr, d_cursor, m->d_row, m->d_val);
         }
         HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 10, d_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -164,6 +178,7 @@ extern "C" int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, co
         return HH_OK;
     }();
     hh_dfree(d_tail);
+    hh_dfree(d_ul);
     hh_dfree(d_cnt);
     if (rc != HH_OK) {
         hh_matrix_destroy(m);

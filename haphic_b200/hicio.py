@@ -197,3 +197,51 @@ def write_bam(path, ref_names, ref_lengths, records, sort_order="unsorted", read
         for i in range(0, len(raw), 0xFF00):
             f.write(_bgzf_block(raw[i:i + 0xFF00]))
         f.write(_bgzf_block(b""))
+
+
+_AS_FMT = {"c": "<b", "C": "<B", "s": "<h", "S": "<H", "i": "<i", "I": "<I"}
+_CIGAR_OPS = "MIDNSHP=X"
+
+
+def write_ul_bam(path, ref_names, ref_lengths, records, repeat=1, random_seq=None):
+    """Single-end BAM writer for ultra-long read fixtures.  Every record is a dict: ``name``, ``flag``, ``ref`` (index, -1 =
+    none), ``pos`` (0-based), ``mapq``, ``cigar`` (a string such as "500S12000M300H"), ``seq`` (False writes SEQ as `*`,
+    i.e. l_seq = 0) and optionally ``AS`` = (value, aux type among c C s S i I).  ``repeat`` writes the compressed records
+    that many times (large files for throughput measurements); ``random_seq`` (a numpy Generator) fills SEQ and QUAL with
+    random bases and qualities, which compress about as well as real reads do (a constant SEQ would not)."""
+    import re
+    out = io.BytesIO()
+    text = "@HD\tVN:1.6\tSO:unsorted\n" + "".join("@SQ\tSN:{}\tLN:{}\n".format(n, l) for n, l in zip(ref_names, ref_lengths))
+    tb = text.encode()
+    out.write(b"BAM\x01" + struct.pack("<i", len(tb)) + tb + struct.pack("<i", len(ref_names)))
+    for n, l in zip(ref_names, ref_lengths):
+        nb = n.encode() + b"\x00"
+        out.write(struct.pack("<i", len(nb)) + nb + struct.pack("<i", int(l)))
+    header = out.getvalue()
+    out = io.BytesIO()
+    for r in records:
+        ops = [(int(ln), _CIGAR_OPS.index(op)) for ln, op in re.findall(r"(\d+)([MIDNSHP=X])", r["cigar"])]
+        l_seq = sum(ln for ln, op in ops if op in (0, 1, 4, 7, 8)) if r.get("seq", True) else 0
+        name = r["name"].encode() + b"\x00"
+        core = struct.pack("<iiBBHHHiiii", int(r["ref"]), int(r["pos"]), len(name), int(r["mapq"]), 4680, len(ops), int(r["flag"]),
+                           l_seq, -1, -1, 0)
+        cigar = b"".join(struct.pack("<I", (ln << 4) | op) for ln, op in ops)
+        if random_seq is None:
+            seq = bytes([0x11] * ((l_seq + 1) // 2)) + bytes([0xFF] * l_seq)
+        else:
+            codes = np.array([1, 2, 4, 8], np.uint8)[random_seq.integers(0, 4, 2 * ((l_seq + 1) // 2))]
+            seq = ((codes[0::2] << 4) | codes[1::2]).tobytes() + random_seq.integers(0, 41, l_seq).astype(np.uint8).tobytes()
+        aux = b""
+        if r.get("AS") is not None:
+            value, typ = r["AS"]
+            aux = b"AS" + typ.encode() + struct.pack(_AS_FMT[typ], int(value))
+        body = core + name + cigar + seq + aux
+        out.write(struct.pack("<i", len(body)) + body)
+    raw = out.getvalue()
+    body = b"".join(_bgzf_block(raw[i:i + 0xFF00]) for i in range(0, len(raw), 0xFF00))
+    with open(path, "wb") as f:
+        for i in range(0, len(header), 0xFF00):
+            f.write(_bgzf_block(header[i:i + 0xFF00]))
+        for _ in range(repeat):
+            f.write(body)
+        f.write(_bgzf_block(b""))

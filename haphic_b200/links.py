@@ -181,18 +181,36 @@ class LinkTable:
         return index, int(n_linked.value)
 
     def to_matrix(self, keep, tail=None, normalize_by_nlinks: bool = False, add_self_loops: bool = True, hap=None,
-                  phasing_weight: float = 0.0) -> "LinkMatrix":
-        """dict_to_matrix on the device; ``hap`` / ``phasing_weight`` as in linked_index."""
+                  phasing_weight: float = 0.0, ul=None) -> "LinkMatrix":
+        """dict_to_matrix on the device; ``hap`` / ``phasing_weight`` as in linked_index.  ``ul`` = (ul_path, ul_parent) per
+        fragment doubles the flank links between two different contigs of one ultra-long-read path
+        (hh_matrix_from_links_ex); the first-seen indices do not depend on it."""
         if self.info is None:
             self.finish()
         keep = np.ascontiguousarray(keep, dtype=np.uint8)
         tail = np.ascontiguousarray(tail if tail is not None else [], dtype=np.int32)
         hap = self._hap(hap)
+        ul_path = ul_parent = None
+        if ul is not None:
+            ul_path, ul_parent = (np.ascontiguousarray(a, dtype=np.int32) for a in ul)
+            if ul_path.shape != (self.n_ctg,) or ul_parent.shape != (self.n_ctg,):
+                raise ValueError("ul_path and ul_parent must have one entry per fragment of the table")
         h = C.c_void_p()
-        check(load().hh_matrix_from_links_phased(self._h, ptr(keep), ptr(tail) if len(tail) else None, len(tail),
-                                                 int(bool(normalize_by_nlinks)), int(bool(add_self_loops)),
-                                                 ptr(hap) if hap is not None else None, float(phasing_weight), C.byref(h)))
+        check(load().hh_matrix_from_links_ex(self._h, ptr(keep), ptr(tail) if len(tail) else None, len(tail),
+                                             int(bool(normalize_by_nlinks)), int(bool(add_self_loops)),
+                                             ptr(hap) if hap is not None else None, float(phasing_weight),
+                                             ptr(ul_path) if ul is not None else None, ptr(ul_parent) if ul is not None else None,
+                                             C.byref(h)))
         return LinkMatrix(self.ctx, h)
+
+    def set_ul_pairs(self, key_i, key_j, ht_slot):
+        """Contig pairs joined by ultra-long reads (hh_links_set_ul_pairs): fetch and fetch_phased then return their full
+        count, and fetch their HT slot ``ht_slot`` (2 * ti + tj), doubled."""
+        ki, kj, hs = (np.ascontiguousarray(a, dtype=np.int32) for a in (key_i, key_j, ht_slot))
+        n = len(ki)
+        if not (len(kj) == len(hs) == n):
+            raise ValueError("key_i, key_j and ht_slot must have the same length")
+        check(load().hh_links_set_ul_pairs(self._h, ptr(ki) if n else None, ptr(kj) if n else None, ptr(hs) if n else None, n))
 
     # -- multi-GPU -------------------------------------------------------------------------
     def export(self):

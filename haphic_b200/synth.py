@@ -332,3 +332,171 @@ def gfa_case(nchr, n_contigs, mean_len, n_pairs, seed, ploidy, n_gfa, chimeras, 
     gfa = [os.path.join(out_dir, "h{}.gfa".format(k + 1)) for k in range(n_gfa)]
     write_gfa(asm, gfa, seed=seed + 4, hap=hap, ploidy=ploidy)
     return gfa
+
+
+def _ul_cigar(q0, q1, read_len, reverse, clip):
+    """CIGAR of an alignment of query [q0, q1) of a read of ``read_len`` bases (reverse: in reference orientation)."""
+    left, right = (read_len - q1, q0) if reverse else (q0, read_len - q1)
+    return "".join("{}{}".format(n, op) for n, op in ((left, clip), (q1 - q0, "M"), (right, clip)) if n)
+
+
+def ul_read(name, a, b, read_no=0, gap=50, span=12000, as_types="iI", rng=None):
+    """Records of one ultra-long read across a junction: ``a`` and ``b`` are (ref index, ref length, reverse) of the two
+    parts in read order.  The primary is one part (a, or b when ``read_no`` is odd), the supplementary the other, with
+    SEQ `*`; the first part is soft-clipped, a forward supplementary sometimes hard-clipped."""
+    rng = rng or np.random.default_rng(read_no)
+    m_a, m_b = min(span, a[1]), min(span, b[1])
+    qa = (100, 100 + m_a)
+    qb = (qa[1] + gap, qa[1] + gap + m_b)
+    read_len = qb[1] + 100
+    parts = []
+    for k, ((ref, ln, rev), q, m, first) in enumerate(((a, qa, m_a, True), (b, qb, m_b, False))):
+        # the first part of the read sits at its contig's right end when forward, the second at the left end
+        pos = (ln - m if not rev else 0) if first else (0 if not rev else ln - m)
+        parts.append(dict(ref=ref, pos=pos, q=q, rev=rev))
+    prim, supp = (parts[1], parts[0]) if read_no % 2 else (parts[0], parts[1])
+    hard = not supp["rev"] and rng.random() < 0.5
+    recs = [dict(name=name, flag=16 if prim["rev"] else 0, ref=prim["ref"], pos=prim["pos"], mapq=60,
+                 cigar=_ul_cigar(*prim["q"], read_len, prim["rev"], "S"), seq=True, AS=(int(rng.integers(0, 30000)), "i")),
+            dict(name=name, flag=0x800 | (0x10 if supp["rev"] else 0), ref=supp["ref"], pos=supp["pos"], mapq=60,
+                 cigar=_ul_cigar(*supp["q"], read_len, supp["rev"], "H" if hard else "S"), seq=hard,
+                 AS=(int(rng.integers(0, 120)), str(rng.choice(list(as_types)))))]
+    return recs
+
+
+def ul_reads(asm, seed, support=3, keep=0.7, detour=None):
+    """Ultra-long reads across the junctions of consecutive contigs of every chromosome: a junction is covered with
+    probability ``keep`` by ``support`` reads (one read, below the default --min_ul_support, otherwise).  Every contig
+    keeps one strand (its orientation), so the semi-contig edges of a chromosome form a chain.  ``detour`` = (contig,
+    length) routes the first covered junction through an extra BAM reference of that name that is not in the FASTA.
+    Returns (reference names, reference lengths, records)."""
+    rng = np.random.default_rng(seed)
+    names, lengths = list(asm.names), [int(x) for x in asm.lengths.tolist()]
+    if detour:
+        names.append(detour[0])
+        lengths.append(int(detour[1]))
+    recs = []
+    n_read = 0
+    for c in range(asm.n - 1):
+        if asm.chrom[c] != asm.chrom[c + 1]:
+            continue
+        a = (c, lengths[c], bool(asm.ori[c]))
+        b = (c + 1, lengths[c + 1], bool(asm.ori[c + 1]))
+        hops = [(a, b)]
+        if detour and n_read == 0:
+            x = (len(names) - 1, lengths[-1], False)
+            hops = [(a, x), (x, b)]
+        n_reads = support if rng.random() < keep else 1
+        for a_, b_ in hops:
+            for _ in range(n_reads):
+                recs += ul_read("ul{}".format(n_read), a_, b_, read_no=n_read, rng=rng)
+                n_read += 1
+    return names, lengths, recs
+
+
+def ul_case(nchr, n_contigs, mean_len, n_pairs, seed, out_dir, ploidy=1, n_gfa=0, bam=False, no_path=False):
+    """A seeded input set for `haphic cluster --ul` in ``out_dir``: asm.fa, aln.pairs (or aln.bam), ul.bam and, with
+    ``n_gfa``, h1.gfa .. (gfa_case).  ``no_path`` writes UL reads that support no junction.  Returns the GFA paths."""
+    import os
+    from . import hicio
+    gfa = gfa_case(nchr, n_contigs, mean_len, n_pairs, seed, max(1, ploidy), max(1, n_gfa), 0, out_dir, bam=bam)
+    if not n_gfa:
+        for p in gfa:
+            os.remove(p)
+        gfa = []
+    asm = make_assembly(nchr, n_contigs, mean_len, seed=seed)
+    names, lengths, recs = ul_reads(asm, seed + 7, support=1 if no_path else 3, detour=("ul_unplaced_1", 30000))
+    hicio.write_ul_bam(os.path.join(out_dir, "ul.bam"), names, lengths, recs)
+    return gfa
+
+
+def _ul_rec(name, part, read_len, flag_extra=0, clip="S", seq=True):
+    return dict(name=name, flag=flag_extra | (0x10 if part["rev"] else 0), ref=part["ref"], pos=part["pos"],
+                mapq=part.get("mapq", 60), cigar=_ul_cigar(*part["q"], read_len, part["rev"], clip), seq=seq,
+                AS=part.get("AS", (1000, "i")))
+
+
+def ul_adversarial():
+    """(reference names, lengths, records) of UL alignments at the edges of parse_ul_alignments: every filter just on
+    either side of its threshold (MAPQ 30 / 29, length 10000 / 9999, end distance 100 / 101, overlap ratio 0.5 / above,
+    gap 10000 / 10001 -- each as the second of two reads, so it decides whether the pair reaches the default support of 2),
+    AS ties over mixed aux widths, supplementaries on the primary's contig, before their primary and after a failed
+    primary, secondary / unmapped / reverse-supplementary flags, a contig reached from three sides, a ring whose inter
+    edges tie for the lightest, junctions below the support, names with `_` and `_bin`, and a path through a reference
+    that the FASTA lacks."""
+    names = ["a_1", "b_1", "c_bin1", "d_bin", "rep", "e", "f", "g", "r0", "r1", "r2", "r3", "h", "i", "w1", "noFA", "w2"]
+    tests = ["mapq", "len", "dist", "overlap", "gap"]
+    for t in tests:
+        for side in ("pass", "fail"):
+            names += ["{}_{}_p".format(t, side), "{}_{}_q".format(t, side)]
+    names += ["tie_p", "tie_q", "tie_z"]
+    lengths = [50000] * len(names)
+    ix = {n: k for k, n in enumerate(names)}
+    rng = np.random.default_rng(77)
+    recs = []
+    count = [0]
+
+    def junction(x, y, n=3, rev=(False, False)):
+        for _ in range(n):
+            recs.extend(ul_read("j{}".format(count[0]), (ix[x], 50000, rev[0]), (ix[y], 50000, rev[1]), read_no=count[0],
+                                as_types="cCsSiI", rng=rng))
+            count[0] += 1
+
+    for x, y in (("a_1", "b_1"), ("b_1", "c_bin1"), ("c_bin1", "d_bin")):
+        junction(x, y, rev=(x == "b_1", False))
+    for x in ("e", "f", "g"):
+        junction(x, "rep")
+    for x, y in (("r0", "r1"), ("r1", "r2"), ("r2", "r3"), ("r3", "r0")):
+        junction(x, y)
+    junction("h", "i", n=1)
+    junction("w1", "noFA")
+    junction("noFA", "w2")
+
+    def pair_read(name, p, s, extra=()):
+        read_len = max(p["q"][1], s["q"][1]) + 100
+        recs.append(_ul_rec(name, p, read_len))
+        recs.append(_ul_rec(name, s, read_len, 0x800, seq=False))
+        for e in extra:
+            recs.append(_ul_rec(name, e, read_len, 0x800, seq=False))
+
+    for t in tests:
+        for side in ("pass", "fail"):
+            pn, qn = ix["{}_{}_p".format(t, side)], ix["{}_{}_q".format(t, side)]
+            junction(names[pn], names[qn], n=1)
+            ok = side == "pass"
+            prim = dict(ref=pn, pos=50000 - 12000, q=(100, 12100), rev=False)
+            supp = dict(ref=qn, pos=0, q=(12150, 24150), rev=False)
+            if t == "mapq":
+                supp["mapq"] = 30 if ok else 29
+            elif t == "len":
+                m = 10000 if ok else 9999
+                supp["q"] = (12150, 12150 + m)
+            elif t == "dist":
+                supp["pos"] = 100 if ok else 101
+            elif t == "overlap":
+                q0 = 6100 if ok else 6099
+                supp["q"] = (q0, q0 + 12000)
+            else:
+                q0 = 22098 if ok else 22099
+                supp["q"] = (q0, q0 + 12000)
+            pair_read("t_{}_{}".format(t, side), prim, supp)
+    # AS ties: two supplementaries with the same score, the first one counts
+    for k, (t1, t2) in enumerate((("c", "S"), ("s", "I"), ("C", "i"))):
+        prim = dict(ref=ix["tie_p"], pos=38000, q=(100, 12100), rev=False, AS=(5000, "I"))
+        s1 = dict(ref=ix["tie_q"], pos=0, q=(12150, 24150), rev=False, AS=(100, t1))
+        s2 = dict(ref=ix["tie_z"], pos=0, q=(12150, 24150), rev=False, AS=(100, t2))
+        pair_read("tie{}".format(k), prim, s1, extra=(s2,))
+    # a supplementary before its primary, one on the primary's own contig, and the supplementaries of a failed primary
+    p = dict(ref=ix["h"], pos=38000, q=(100, 12100), rev=False)
+    s = dict(ref=ix["i"], pos=0, q=(12150, 24150), rev=False)
+    recs.append(_ul_rec("early", s, 24250, 0x800, seq=False))
+    recs.append(_ul_rec("early", p, 24250))
+    recs.append(_ul_rec("early", dict(p, pos=0), 24250, 0x800, seq=False))
+    recs.append(_ul_rec("weak", dict(p, mapq=5), 24250))
+    recs.append(_ul_rec("weak", s, 24250, 0x800, seq=False))
+    recs.append(_ul_rec("weak", s, 24250, 0x800, seq=False))
+    # flags that are neither primary nor supplementary, and an unmapped record
+    recs.append(_ul_rec("early", s, 24250, 0x100, seq=False))
+    recs.append(dict(_ul_rec("early", s, 24250, 0x4), ref=-1, pos=-1))
+    recs.append(_ul_rec("dup", p, 24250, 0x400))
+    return names, lengths, recs

@@ -127,6 +127,13 @@ int hh_links_fetch(hh_links* lk, int32_t* key_i, int32_t* key_j, uint32_t* full,
  * entries, of which the first *n_out are written. */
 int hh_links_fetch_phased(hh_links* lk, const int32_t* hap, double w, int32_t* key_i, int32_t* key_j, double* values,
                           uint8_t* is_float, int64_t* n_out);
+/* The contig pairs that ultra-long reads join (add_HT_links_based_on_ul 1912-1933 and the full links of
+ * add_flank_and_full_links_based_on_ul 1936-1985): key_i / key_j [n_pairs] (host) as in hh_links_fetch (name(key_i) <
+ * name(key_j)), ht_slot the HT_link_dict slot 2 * ti + tj of the joined semi-contigs.  From then on hh_links_fetch returns
+ * those entries with the full count and that HT slot doubled (HH still derived from the stored counts) and
+ * hh_links_fetch_phased doubles the full count before the reduction; the stored counts are not changed.  A doubled count
+ * above 2^32 - 1 fails the fetch.  Pairs absent from the table are ignored; n_pairs = 0 detaches the list. */
+int hh_links_set_ul_pairs(hh_links* lk, const int32_t* key_i, const int32_t* key_j, const int32_t* ht_slot, int64_t n_pairs);
 /* ctg_link_dict (1638-1639): per-contig flank-link totals, [n_ctg] */
 int hh_links_fetch_ctg(hh_links* lk, int64_t* ctg_links);
 /* multi-GPU: export the finished table as device arrays / merge a peer's export into this
@@ -176,6 +183,15 @@ int hh_links_linked_index_phased(hh_links* lk, const uint8_t* keep, int normaliz
                                  int32_t* index, int32_t* n_linked);
 int hh_matrix_from_links_phased(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
                                 int normalize_by_nlinks, int add_self_loops, const int32_t* hap, double w, hh_matrix** out);
+/* hh_matrix_from_links_phased with the ultra-long-read boost of add_flank_and_full_links_based_on_ul (1936-1985): ul_path and
+ * ul_parent [n_ctg] (host) give every fragment of the table the path id of its contig (-1 = on no path) and the id of its
+ * contig (a bin's parent).  An entry whose ends lie on two different contigs of one path counts twice, after normalisation
+ * and before the phasing reduction.  Doubling deletes no entry, so the first-seen indices are those of
+ * hh_links_linked_index_phased with the same keep / normalize_by_nlinks / hap / w.  ul_path = NULL is
+ * hh_matrix_from_links_phased. */
+int hh_matrix_from_links_ex(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail, int normalize_by_nlinks,
+                            int add_self_loops, const int32_t* hap, double w, const int32_t* ul_path, const int32_t* ul_parent,
+                            hh_matrix** out);
 /* rank-sum statistic of filter_fragments, HapHiC_cluster.py:864-892, on a matrix WITHOUT self loops: for every
  * fragment, sort its row by links descending (ties by matrix index, a stable list.sort(reverse=True)), take
  * the first topN fragments and sum min(rank_a(b), rank_b(a)) over their pairs.  rank_sum[n] (host) is
@@ -394,6 +410,20 @@ int hh_bam_open(const char* path, const char* names_blob, int32_t n_names, int i
 int hh_bam_header_text(hh_bam_reader* r, const char** text, int64_t* len);
 int hh_bam_next(hh_bam_reader* r, int32_t* rec, int64_t max_records, int64_t* n_out);
 int hh_bam_close(hh_bam_reader* r);
+/* Ultra-long read alignments (`--ul`, parse_ul_alignments 1763-1869): hh_ul_open reads the whole BAM once (BGZF inflated
+ * on `threads` threads) with the htslib filter !flag.unmap, drops alignments with MAPQ < min_mapq, reference length <
+ * min_alignment_length or more than max_distance_to_end from both ends of the reference (lengths from the BAM header), and
+ * runs the primary (flag 0 / 16) / supplementary (0x800, same read, other reference, query-interval overlap and gap tests)
+ * state machine; each primary with accepted supplementaries yields one event from the one with the highest AS (first on a
+ * tie).  hh_ul_info / hh_ul_fetch hand out the header's references (names NUL-separated, names_bytes in all, lengths) and
+ * the events [n_events][4] in file order: left semi-contig, right semi-contig (2 * reference index + 0 for `_H`, 1 for
+ * `_T`), primary reference, supplementary reference.  Any output pointer may be NULL. */
+typedef struct hh_ul_reader hh_ul_reader;
+int hh_ul_open(const char* path, int threads, int32_t min_mapq, int64_t min_alignment_length, int64_t max_distance_to_end,
+               double max_overlap_ratio, int64_t max_gap_len, hh_ul_reader** out);
+int hh_ul_info(hh_ul_reader* r, int32_t* n_ref, int64_t* names_bytes, int64_t* n_events, int64_t* n_records);
+int hh_ul_fetch(hh_ul_reader* r, char* names, int64_t* ref_len, int32_t* events);
+int hh_ul_close(hh_ul_reader* r);
 
 /* paired_links.clm straight from the record stream (update_clm_dict 395-401 + output_clm 376-392): for every contig
  * pair with >= 2 links, in dict insertion order, four lines (orientations ++ +- -+ --)
