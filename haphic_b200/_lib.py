@@ -130,7 +130,21 @@ _SIGNATURES = {
     "hh_correct_set_layout": (C.c_int, [_P, _P, _P, _P, C.c_int32]),
     "hh_correct_remap": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int]),
     "hh_correct_destroy": (C.c_int, [_P]),
-    "hh_pairs_open": (C.c_int, [C.c_char_p, _P, C.c_int32, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
+    "hh_contact_create": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int64, C.POINTER(_P)]),
+    "hh_contact_load": (C.c_int, [_P, C.c_int32, _P, C.POINTER(_P)]),
+    "hh_contact_add": (C.c_int, [_P, _P, C.c_int64, C.c_int]),
+    "hh_contact_add_async": (C.c_int, [_P, _P, C.c_int64]),
+    "hh_contact_error": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                   C.POINTER(C.c_int64)]),
+    "hh_contact_finish": (C.c_int, [_P]),
+    "hh_contact_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    "hh_contact_fetch": (C.c_int, [_P, _P]),
+    "hh_contact_kr": (C.c_int, [_P, C.c_int32, _P, _P, C.c_double, C.c_double, C.c_double, C.c_int32, C.c_int32, _P, _P,
+                                _P, _P]),
+    "hh_contact_normalize": (C.c_int, [_P, C.c_int, C.c_int32, _P, _P, _P, _P, _P, C.POINTER(C.c_double),
+                                       C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
+    "hh_contact_destroy": (C.c_int, [_P]),
+    "hh_pairs_open":(C.c_int, [C.c_char_p, _P, C.c_int32, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
     "hh_pairs_next": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "hh_pairs_close": (C.c_int, [_P]),
     "hh_pairs_write": (C.c_int, [C.c_char_p, _P, C.c_int32, _P, C.c_int64, C.c_int64, C.c_int, C.c_int]),

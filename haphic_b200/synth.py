@@ -500,3 +500,27 @@ def ul_adversarial():
     recs.append(dict(_ul_rec("early", s, 24250, 0x4), ref=-1, pos=-1))
     recs.append(_ul_rec("dup", p, 24250, 0x400))
     return names, lengths, recs
+
+
+def write_agp(asm: Assembly, path: str, gap: int = 100, prefix: str = "group") -> list:
+    """The true layout of ``asm`` as an AGP: one scaffold per chromosome (``{prefix}{c + 1}``), its contigs in order, each
+    W line oriented so that the contig reads along the chromosome ('-' for reverse-complemented ones), with a U gap of
+    ``gap`` bp between neighbours.  Returns the W pieces (scaffold, scaffold start, contig id, orientation) in file order."""
+    pieces = []
+    with open(path, "w") as f:
+        for c in range(asm.nchr):
+            pos, part = 1, 1
+            ids = np.nonzero(asm.chrom == c)[0]
+            for k, i in enumerate(ids.tolist()):
+                if k:
+                    f.write("{}{}\t{}\t{}\t{}\tU\t{}\tscaffold\tyes\tproximity_ligation\n".format(
+                        prefix, c + 1, pos, pos + gap - 1, part, gap))
+                    pos += gap
+                    part += 1
+                ln = int(asm.lengths[i])
+                ori = "-" if asm.ori[i] else "+"
+                f.write("{}{}\t{}\t{}\t{}\tW\t{}\t1\t{}\t{}\n".format(prefix, c + 1, pos, pos + ln - 1, part, asm.names[i], ln, ori))
+                pieces.append((c, pos, i, ori))
+                pos += ln
+                part += 1
+    return pieces

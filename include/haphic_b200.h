@@ -384,6 +384,47 @@ int hh_correct_set_layout(hh_correct* cr, const int32_t* src_base, const int64_t
 int hh_correct_remap(hh_correct* cr, const int32_t* rec_in, int32_t* rec_out, int64_t n_rec, int mem);
 int hh_correct_destroy(hh_correct* cr);
 
+/* ---- contact maps (`haphic plot`, scripts/HapHiC_plot.py v1.0.7) ------------------------- *
+ * The AGP layout is resolved on the host (parse_agp 41-103, generate_contact_matrix 106-150); the device gets, per contig
+ * id, in_set (the contig is in ctg_set) and a dense run of (contig, aln bin) slots: slot_base[c] .. slot_base[c+1]-1 are
+ * aln bins 0, 1, ... of contig c.  cand_off[slot] .. cand_off[slot+1]-1 are that slot's entries of ctg_aln_dict, in list
+ * order: the closed raw range [cand_lo, cand_hi] and the total bin of its ctg_dict mapping (overwrites already resolved),
+ * or -1 when that scaffold is not kept.  An empty slot is an aln bin the contig has no list for (the KeyError).
+ *   hh_contact_create: the nb x nb count matrix (int32 while the records added cannot make a symmetrised entry reach 2^31,
+ *     widened to int64 on the device by the add that would).
+ *   hh_contact_load: a finished handle holding an nb x nb symmetrised int64 count matrix (a `contact_matrix.pkl`,
+ *     load_pickle 266-288), for the KR / normalisation calls.
+ *   hh_contact_add / hh_contact_add_async: parse_pairs / parse_bam with convert_group_bin_id (153-245) over records
+ *     {id_a, pos_a, id_b, pos_b} (0-based positions, ids < 0 or >= n_ctg are not in ctg_set), in stream order across
+ *     calls.  Host batches are staged through pinned double buffers; _async takes device records and returns at once.
+ *   hh_contact_error: the first offending record in stream order (index -1: none), which end (0 / 1), its contig id and
+ *     1-based position: the reference raises "Cannot find alignment position" for it.
+ *   hh_contact_finish: contact_matrix + contact_matrix.T with the diagonal halved (854-856), in place.
+ *   hh_contact_info / hh_contact_fetch: nb, bytes per stored count, records added; the symmetrised counts as int64.
+ *   hh_contact_kr: bnewt (291-404) on n_prob diagonal blocks (off, n) of counts + 1e-5, all advanced together;
+ *     x_out holds the problems' x one after the other, status 1 = "Unable to converge" (1000 outer / 10000 inner steps).
+ *   hh_contact_normalize: normalize_matrix (407-504).  mode 0 = KR: x_whole[i] A_ij x_whole[j], replaced inside the blocks
+ *     by x_blocks (indexed by bin), 0 where the count is 0; 1 = log10(count + 1); 2 = counts.  out (nb x nb fp64 host
+ *     array, may be NULL) gets the matrix; the off-diagonal block entries (unmasked) are sorted on the device and their
+ *     median's two middle values (equal for an odd count) returned with the count. */
+typedef struct hh_contact hh_contact;
+int hh_contact_create(hh_ctx* ctx, int32_t n_ctg, const uint8_t* in_set, const int64_t* slot_base, const int64_t* cand_off,
+                      const int64_t* cand_lo, const int64_t* cand_hi, const int32_t* cand_bin, int32_t nb, int64_t bin_size,
+                      hh_contact** out);
+int hh_contact_load(hh_ctx* ctx, int32_t nb, const int64_t* counts, hh_contact** out);
+int hh_contact_add(hh_contact* h, const int32_t* rec, int64_t n_rec, int mem);
+int hh_contact_add_async(hh_contact* h, const int32_t* rec_dev, int64_t n_rec);
+int hh_contact_error(hh_contact* h, int64_t* index, int32_t* end, int32_t* ctg, int64_t* pos);
+int hh_contact_finish(hh_contact* h);
+int hh_contact_info(hh_contact* h, int32_t* nb, int32_t* count_bytes, int64_t* n_records);
+int hh_contact_fetch(hh_contact* h, int64_t* out);
+int hh_contact_kr(hh_contact* h, int32_t n_prob, const int32_t* off, const int32_t* n, double tol, double delta, double Delta,
+                  int32_t max_outer, int32_t max_inner, double* x_out, int32_t* n_outer, int64_t* n_inner, int32_t* status);
+int hh_contact_normalize(hh_contact* h, int mode, int32_t n_blk, const int32_t* blk_off, const int32_t* blk_n,
+                         const double* x_blocks, const double* x_whole, double* out, double* median_lo, double* median_hi,
+                         int64_t* n_values);
+int hh_contact_destroy(hh_contact* h);
+
 /* ---- host-side I/O around the path (native, no CUDA) ------------------------------------------------
  * .pairs / .pairs.gz reader: pairs_generator / pairs_generator_inter_ctgs, HapHiC_cluster.py:1539-1583.  Skips blank
  * and '#' lines, takes `cols[1], int(cols[2])-1, cols[3], int(cols[4])-1`, writes the two BED lines per pair
