@@ -74,6 +74,7 @@ _SIGNATURES = {
     "hh_links_add_async": (C.c_int, [_P, _P, C.c_int64, C.c_int64]),
     "hh_links_finish": (C.c_int, [_P, C.POINTER(LinksInfo)]),
     "hh_links_agg_info": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "hh_links_record_bytes": (C.c_int, [_P, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "hh_links_fetch": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "hh_links_fetch_phased": (C.c_int, [_P, _P, C.c_double, _P, _P, _P, _P, C.POINTER(C.c_int64)]),
     "hh_links_set_ul_pairs": (C.c_int, [_P, _P, _P, _P, C.c_int64]),

@@ -178,6 +178,11 @@ __device__ __forceinline__ int4 hh_ld_stream(const int4* p) {
                  : "l"(p));
     return r;
 }
+__device__ __forceinline__ unsigned long long hh_ld_stream_u64(const unsigned long long* p) {
+    unsigned long long r;
+    asm volatile("ld.global.nc.L1::no_allocate.u64 %0, [%1];" : "=l"(r) : "l"(p));
+    return r;
+}
 __device__ __forceinline__ float4 hh_ld_stream_f4(const float4* p) {
     float4 r;
     asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"

@@ -29,7 +29,8 @@ struct __align__(32) hh_slot {
 };
 
 struct hh_partset {
-    int4* buf;                       // [npart][pcap] records {i, j, stream index, flags}
+    void* buf;                       // [npart][pcap] records: hh_nrec when narrow, else int4 (see "partition records")
+    bool narrow;
     unsigned long long* cursor;      // [npart] records written to every region (may exceed pcap: the excess went to the spill list)
     uint64_t pcap;                   // records per partition region
     int64_t sized_for, sent;         // records the set was sized for / sent to it so far
@@ -68,11 +69,14 @@ struct hh_links {
     // partitioned counting (contig mode, long streams; see "partition, then aggregate" below)
     int mode;                        // 0 undecided, 1 direct (one big hash table), 2 partitioned
     int npart_log;                   // log2 of the number of partitions
+    int kbits;                       // bits of j in the pair key (i << kbits) | j: the least with 2^kbits >= n_ctg
+    std::vector<int32_t> set_bytes;  // record bytes of every partition set opened (hh_links_record_bytes)
+    int32_t bucket_bytes;            // record bytes of the bucket buffer of the finish, 0 before it
     uint64_t scap;                   // slots of a shared-memory table, or of the fallback's global table when one ran
     int64_t agg_buckets, agg_smem, agg_fallback;   // buckets at finish / counted in shared memory / by the fallback
     uint64_t spill_cap;
     std::vector<hh_partset> psets;   // partition buffers; normally one set, a new one when a later add call outgrows it
-    int4* d_spill;                   // records of partitions whose region overflowed (skewed keys), with their partition id
+    int4* d_spill;                   // wide records of partitions whose region overflowed (skewed keys)
     unsigned long long* d_spill_cursor;
     int64_t capacity_hint;
     // dict_to_matrix support
@@ -384,7 +388,7 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 // (about 1.3k records at the benchmark's 200M records) is then sorted by pair in shared memory, its runs are reduced, and
 // it is emitted as compact entries (9 words, the hh_links_adopt list format).  Integer adds and mins only: the result is identical to
 // the direct path.
-//   hh_k_part_scatter   record -> {i, j, stream index, flags} (ends ordered by name rank, is_flank / head-tail evaluated once)
+//   hh_k_part_scatter   record -> partition record (ends ordered by name rank, is_flank / head-tail evaluated once)
 //   hh_k_part_hist      records per bucket (shared-memory histogram of a region's sub-buckets per tile)
 //   hh_k_part_scatter2  the same pass again: every record to its place in the dense bucket buffer
 //   hh_k_bucket_count   persistent CTAs: count one bucket at a time in shared memory (sort by pair, reduce the runs),
@@ -392,12 +396,59 @@ hh_k_links_insert(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 //   hh_k_part_step      fallback for the buckets shared memory does not take: gathered, then counted in batches of
 //                       about 2^19 records through global scratch tables
 // ---------------------------------------------------------------------------------------------
-#define HH_PART_TILE 4096          // records per tile of the scatter kernel (512 threads x 8)
+#define HH_PART_TILE 4096          // wide records per tile of the scatter kernels (512 threads x 8), and spill records per tile
 #define HH_PART_MAX 1024
+
+// ---- partition records ------------------------------------------------------------------------------------------------
+// Every usable record crosses device memory four times between the scatter and the count, so its width sets the cost of
+// those passes.  Two formats:
+//   wide   int4 {i, j, stream index, flags | partition << 8}: any key space and stream index (the partition is only
+//          read by the scatter that wrote it, and is absent from records converted from the narrow format);
+//   narrow hh_nrec, 8 bytes: high word the pair key (i << kbits) | j, low word flags << 29 | stream index.  It holds
+//          what the count needs while kbits <= 16 (at most 65,536 objects) and stream indices are below 2^29.  Its
+//          partition is not stored: the region it sits in implies it, and hh_bucket_of recomputes it from the key.
+// A partition set is narrow when the call that opens it can use the narrow format (links_narrow); the bucket buffer of
+// the finish is narrow when the whole stream can.  The spill list, shared by all sets and rarely used, stays wide.
+#define HH_NREC_KBITS 16
+#define HH_NREC_ZBITS 29
+#define HH_NREC_ZEND (1ll << HH_NREC_ZBITS)     // narrow records carry stream indices below this
+
+struct __align__(8) hh_nrec {
+    unsigned long long v;
+};
+
+__device__ __forceinline__ int4 hh_ld_rec(const int4* p) { return hh_ld_stream(p); }
+__device__ __forceinline__ hh_nrec hh_ld_rec(const hh_nrec* p) { return hh_nrec{hh_ld_stream_u64(&p->v)}; }
+
+__device__ __forceinline__ uint32_t hh_rec_i(int4 r, int) { return (uint32_t)r.x; }
+__device__ __forceinline__ uint32_t hh_rec_j(int4 r, int) { return (uint32_t)r.y; }
+__device__ __forceinline__ uint32_t hh_rec_z(int4 r) { return (uint32_t)r.z; }
+__device__ __forceinline__ unsigned hh_rec_flags(int4 r) { return (unsigned)r.w & 7u; }
+__device__ __forceinline__ uint32_t hh_rec_i(hh_nrec r, int kbits) { return (uint32_t)(r.v >> 32) >> kbits; }
+__device__ __forceinline__ uint32_t hh_rec_j(hh_nrec r, int kbits) { return (uint32_t)(r.v >> 32) & ((1u << kbits) - 1u); }
+__device__ __forceinline__ uint32_t hh_rec_z(hh_nrec r) { return (uint32_t)r.v & (uint32_t)(HH_NREC_ZEND - 1); }
+__device__ __forceinline__ unsigned hh_rec_flags(hh_nrec r) { return (uint32_t)r.v >> HH_NREC_ZBITS; }
+
+__device__ __forceinline__ hh_nrec hh_nrec_make(uint32_t i, uint32_t j, uint32_t z, unsigned flags, int kbits) {
+    return hh_nrec{((unsigned long long)((i << kbits) | j) << 32) | ((unsigned long long)flags << HH_NREC_ZBITS) | z};
+}
+
+// *d = s in the format of d
+__device__ __forceinline__ void hh_rec_put(int4* d, int4 s, int) { *d = s; }
+__device__ __forceinline__ void hh_rec_put(hh_nrec* d, hh_nrec s, int) { *d = s; }
+__device__ __forceinline__ void hh_rec_put(int4* d, hh_nrec s, int kbits) {
+    *d = make_int4((int)hh_rec_i(s, kbits), (int)hh_rec_j(s, kbits), (int)hh_rec_z(s), (int)hh_rec_flags(s));
+}
+__device__ __forceinline__ void hh_rec_put(hh_nrec* d, int4 s, int kbits) {
+    *d = hh_nrec_make(hh_rec_i(s, kbits), hh_rec_j(s, kbits), hh_rec_z(s), hh_rec_flags(s), kbits);
+}
+
+__device__ __forceinline__ void hh_rec_set_z(int4* r, uint32_t z) { r->z = (int)z; }
+__device__ __forceinline__ void hh_rec_set_z(hh_nrec* r, uint32_t z) { r->v = (r->v & ~(unsigned long long)(HH_NREC_ZEND - 1)) | z; }
 
 // The scatter kernels stage a tile's records in dynamic shared memory, ordered by destination (partition, or sub-bucket),
 // so that consecutive threads store the consecutive records of one run: a warp store then covers a few contiguous
-// stretches instead of 32 lines.  64 KiB per CTA beside 12 or 32 KiB of static arrays: two CTAs per SM, as the 62 / 63
+// stretches instead of 32 lines.  64 KiB per CTA beside 12 or 32 KiB of static arrays: two CTAs per SM, as the
 // registers x 512 threads allow anyway.
 #define HH_STAGE_SMEM ((size_t)HH_PART_TILE * sizeof(int4))
 
@@ -436,35 +487,60 @@ __device__ __forceinline__ unsigned int hh_tile_scan(unsigned int* c, int n, uns
     return all;
 }
 
+// A bucket (or a partition: bucket_log = npart_log) is the top bucket_log bits of hh_mix64(key).
+template <typename R>
+__device__ __forceinline__ uint32_t hh_bucket_of(R r, int bucket_log, int kbits) {
+    return (uint32_t)(hh_mix64(hh_pair_key((int)hh_rec_i(r, kbits), (int)hh_rec_j(r, kbits))) >> (64 - bucket_log));
+}
+
+// partition records of the scatter, and the partition of a staged one
+__device__ __forceinline__ void hh_part_rec(int4* o, const hh_pair& pr, uint32_t z, unsigned p, int) {
+    *o = make_int4(pr.a, pr.b, (int)z, (int)(pr.flags | (p << 8)));
+}
+__device__ __forceinline__ void hh_part_rec(hh_nrec* o, const hh_pair& pr, uint32_t z, unsigned, int kbits) {
+    *o = hh_nrec_make((uint32_t)pr.a, (uint32_t)pr.b, z, pr.flags, kbits);
+}
+__device__ __forceinline__ unsigned hh_part_of(int4 r, int, int) { return (unsigned)r.w >> 8; }
+__device__ __forceinline__ unsigned hh_part_of(hh_nrec r, int npart_log, int kbits) { return hh_bucket_of(r, npart_log, kbits); }
+
+// records per tile of hh_k_part_scatter: the 64 KiB of staging, 512 threads x 8 wide or 16 narrow records (a run of a
+// partition is then about 128 B long at 512 partitions either way)
+template <typename R>
+__host__ __device__ constexpr int hh_scatter_tile() { return (int)(HH_STAGE_SMEM / sizeof(R)); }
+
+template <typename R>
 __global__ void __launch_bounds__(512, 2)
 hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_off, int32_t n_ctg, const int32_t* __restrict__ ctg_len,
-                  const int32_t* __restrict__ name_rank, const uint8_t* __restrict__ in_nx, int64_t flank_bp, int npart_log,
-                  int4* __restrict__ pbuf, uint64_t pcap, unsigned long long* __restrict__ cursor, int4* __restrict__ spill,
+                  const int32_t* __restrict__ name_rank, const uint8_t* __restrict__ in_nx, int64_t flank_bp, int npart_log, int kbits,
+                  R* __restrict__ pbuf, uint64_t pcap, unsigned long long* __restrict__ cursor, int4* __restrict__ spill,
                   uint64_t spill_cap, unsigned long long* __restrict__ spill_cursor, unsigned long long* __restrict__ counters) {
-    extern __shared__ int4 s_stage[];                // HH_PART_TILE records, ordered by partition
+    constexpr int TILE = hh_scatter_tile<R>(), ITEMS = TILE / 512;
+    extern __shared__ int4 s_stage_mem[];
+    R* s_stage = reinterpret_cast<R*>(s_stage_mem);  // TILE records, ordered by partition
     __shared__ unsigned int s_cnt[HH_PART_MAX];      // records of the tile per partition, then their exclusive prefix
     __shared__ unsigned long long s_base[HH_PART_MAX];
     __shared__ unsigned int s_wtot[16];
     __shared__ unsigned int s_used;
     const int npart = 1 << npart_log;
-    const int64_t tiles = (n_rec + HH_PART_TILE - 1) / HH_PART_TILE;
+    const int64_t tiles = (n_rec + TILE - 1) / TILE;
     unsigned int my_used = 0;
     if (threadIdx.x == 0) s_used = 0;
     for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
         for (int k = threadIdx.x; k < npart; k += 512) s_cnt[k] = 0;
         __syncthreads();
-        int4 out[8];
-        unsigned int rnk[8];                            // rank in the tile's run of its partition (.w >> 8), ~0 = none
+        // Until it is staged, a record holds partition << 13 | its rank in the tile's run of that partition (< 2^13) in
+        // place of its stream index, which its place in the tile implies: no registers beside the records.
+        R out[ITEMS];
+        uint32_t live = 0;                              // bit k: out[k] holds a record
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const int64_t i = t * HH_PART_TILE + (int64_t)k * 512 + threadIdx.x;
-            rnk[k] = HH_NONE32;
+        for (int k = 0; k < ITEMS; ++k) {
+            const int64_t i = t * TILE + (int64_t)k * 512 + threadIdx.x;
             if (i < n_rec) {
                 hh_pair pr;
                 if (hh_classify_contig(hh_ld_stream(rec + i), n_ctg, ctg_len, name_rank, in_nx, flank_bp, &pr)) {
-                    const int p = (int)(hh_mix64(hh_pair_key(pr.a, pr.b)) >> (64 - npart_log));
-                    rnk[k] = atomicAdd(&s_cnt[p], 1u);
-                    out[k] = make_int4(pr.a, pr.b, (int)(stream_off + (uint32_t)i), (int)(pr.flags | ((unsigned)p << 8)));
+                    const unsigned p = (unsigned)(hh_mix64(hh_pair_key(pr.a, pr.b)) >> (64 - npart_log));
+                    hh_part_rec(&out[k], pr, (p << 13) | atomicAdd(&s_cnt[p], 1u), p, kbits);
+                    live |= 1u << k;
                     my_used++;
                 }
             }
@@ -474,20 +550,24 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
             if (s_cnt[k]) s_base[k] = atomicAdd(cursor + k, (unsigned long long)s_cnt[k]);
         const unsigned int n_tile = hh_tile_scan(s_cnt, npart, s_wtot);
 #pragma unroll
-        for (int k = 0; k < 8; ++k)
-            if (rnk[k] != HH_NONE32) s_stage[s_cnt[(unsigned)out[k].w >> 8] + rnk[k]] = out[k];
+        for (int k = 0; k < ITEMS; ++k) {
+            if (!((live >> k) & 1u)) continue;
+            const uint32_t at = hh_rec_z(out[k]);
+            hh_rec_set_z(&out[k], stream_off + (uint32_t)(t * TILE + k * 512 + threadIdx.x));
+            s_stage[s_cnt[at >> 13] + (at & 0x1FFFu)] = out[k];
+        }
         __syncthreads();
-        // staged record e is number e - s_cnt[p] of the tile's run in partition p (p is in bits 8 and up of .w)
+        // staged record e is number e - s_cnt[p] of the tile's run in partition p
         for (unsigned int e = threadIdx.x; e < n_tile; e += 512) {
-            const int4 r = s_stage[e];
-            const unsigned int p = (unsigned)r.w >> 8;
+            const R r = s_stage[e];
+            const unsigned int p = hh_part_of(r, npart_log, kbits);
             const unsigned long long q = s_base[p] + (e - s_cnt[p]);
             if (q < pcap) {
                 pbuf[(size_t)p * (size_t)pcap + (size_t)q] = r;
             } else {
                 // the region of this partition is full (a few pairs own a large share of the stream): spill list
                 const unsigned long long sq = atomicAdd(spill_cursor, 1ull);
-                if (sq < spill_cap) spill[sq] = r;
+                if (sq < spill_cap) hh_rec_put(spill + sq, r, kbits);
                 else atomicExch(counters + 2, 3ull);
             }
         }
@@ -508,16 +588,14 @@ hh_k_part_scatter(const int4* __restrict__ rec, int64_t n_rec, uint32_t stream_o
 #define HH_AGG_THREADS 256
 #define HH_AGG_HOT 32              // a bucket with more than HH_AGG_HOT x the mean records skips shared memory (links_hot_records)
 
-__device__ __forceinline__ uint32_t hh_bucket_of(int4 r, int bucket_log) {
-    return (uint32_t)(hh_mix64(hh_pair_key(r.x, r.y)) >> (64 - bucket_log));
-}
-
 // Records per bucket.  The virtual tiles are `tpr` tiles of every region (those past the region's fill exit at once),
 // then the spill list; a region tile histograms its 2^(bucket_log - npart_log) sub-buckets in shared memory and adds them
 // with one global atomic per sub-bucket.  Spill records (rare) go straight to their bucket.
+template <typename R>
 __global__ void __launch_bounds__(512)
-hh_k_part_hist(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int64_t tpr,
-               const int4* __restrict__ spill, int64_t n_spill, int bucket_log, unsigned int* __restrict__ bcnt) {
+hh_k_part_hist(const R* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int kbits,
+               int64_t tpr, const int4* __restrict__ spill, int64_t n_spill, int bucket_log, unsigned int* __restrict__ bcnt) {
+    constexpr int TILE = HH_PART_TILE, ITEMS = TILE / 512;
     __shared__ unsigned int s_cnt[1 << HH_SUB_MAX_LOG];
     const int sub_log = bucket_log - npart_log, nsub = 1 << sub_log;
     const int64_t region_tiles = ((int64_t)1 << npart_log) * tpr;
@@ -526,20 +604,20 @@ hh_k_part_hist(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long
         if (t >= region_tiles) {
             const int64_t base = (t - region_tiles) * HH_PART_TILE;
             for (int k = threadIdx.x; k < HH_PART_TILE; k += 512)
-                if (base + k < n_spill) atomicAdd(bcnt + hh_bucket_of(hh_ld_stream(spill + base + k), bucket_log), 1u);
+                if (base + k < n_spill) atomicAdd(bcnt + hh_bucket_of(hh_ld_rec(spill + base + k), bucket_log, kbits), 1u);
             continue;
         }
         const int p = (int)(t / tpr);
-        const uint64_t start = (uint64_t)(t % tpr) * HH_PART_TILE;
+        const uint64_t start = (uint64_t)(t % tpr) * TILE;
         const uint64_t fill = min((uint64_t)cursor[p], pcap);
         if (start >= fill) continue;                    // block-uniform
         for (int k = threadIdx.x; k < nsub; k += 512) s_cnt[k] = 0;
         __syncthreads();
-        const int4* reg = pbuf + (size_t)p * (size_t)pcap;
+        const R* reg = pbuf + (size_t)p * (size_t)pcap;
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
+        for (int k = 0; k < ITEMS; ++k) {
             const uint64_t i = start + (uint64_t)k * 512 + threadIdx.x;
-            if (i < fill) atomicAdd(&s_cnt[hh_bucket_of(hh_ld_stream(reg + i), bucket_log) & (nsub - 1)], 1u);
+            if (i < fill) atomicAdd(&s_cnt[hh_bucket_of(hh_ld_rec(reg + i), bucket_log, kbits) & (nsub - 1)], 1u);
         }
         __syncthreads();
         for (int k = threadIdx.x; k < nsub; k += 512)
@@ -548,14 +626,17 @@ hh_k_part_hist(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long
     }
 }
 
-// The pass of hh_k_part_hist again: every record goes to boff[bucket] + its rank.  Ranks inside a tile come from shared
-// memory, one global atomic per (tile, sub-bucket) reserves the tile's run; bfill counts what each bucket received.  A
-// region tile is staged in shared memory ordered by sub-bucket and stored run by run.
+// The pass of hh_k_part_hist again: every record goes to boff[bucket] + its rank, in the bucket buffer's format D.  Ranks
+// inside a tile come from shared memory, one global atomic per (tile, sub-bucket) reserves the tile's run; bfill counts
+// what each bucket received.  A region tile is staged in shared memory ordered by sub-bucket and stored run by run.
+template <typename R, typename D>
 __global__ void __launch_bounds__(512, 2)
-hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int64_t tpr,
-                   const int4* __restrict__ spill, int64_t n_spill, int bucket_log, const int64_t* __restrict__ boff,
-                   unsigned int* __restrict__ bfill, int4* __restrict__ out, uint64_t n_out, unsigned long long* __restrict__ counters) {
-    extern __shared__ int4 s_stage[];                    // HH_PART_TILE records, ordered by sub-bucket
+hh_k_part_scatter2(const R* __restrict__ pbuf, uint64_t pcap, const unsigned long long* __restrict__ cursor, int npart_log, int kbits,
+                   int64_t tpr, const int4* __restrict__ spill, int64_t n_spill, int bucket_log, const int64_t* __restrict__ boff,
+                   unsigned int* __restrict__ bfill, D* __restrict__ out, uint64_t n_out, unsigned long long* __restrict__ counters) {
+    constexpr int TILE = HH_PART_TILE, ITEMS = TILE / 512;
+    extern __shared__ int4 s_stage_mem[];
+    R* s_stage = reinterpret_cast<R*>(s_stage_mem);      // TILE records, ordered by sub-bucket
     __shared__ unsigned int s_cnt[1 << HH_SUB_MAX_LOG];  // records of the tile per sub-bucket, then their exclusive prefix
     __shared__ unsigned int s_base[1 << HH_SUB_MAX_LOG];
     __shared__ unsigned int s_wtot[16];
@@ -567,30 +648,30 @@ hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned 
             const int64_t base = (t - region_tiles) * HH_PART_TILE;
             for (int k = threadIdx.x; k < HH_PART_TILE; k += 512) {
                 if (base + k >= n_spill) break;
-                const int4 r = hh_ld_stream(spill + base + k);
-                const uint32_t b = hh_bucket_of(r, bucket_log);
+                const int4 r = hh_ld_rec(spill + base + k);
+                const uint32_t b = hh_bucket_of(r, bucket_log, kbits);
                 const uint64_t q = (uint64_t)boff[b] + atomicAdd(bfill + b, 1u);
-                if (q < n_out) out[q] = r;
+                if (q < n_out) hh_rec_put(out + q, r, kbits);
                 else atomicExch(counters + 2, 6ull);
             }
             continue;
         }
         const int p = (int)(t / tpr);
-        const uint64_t start = (uint64_t)(t % tpr) * HH_PART_TILE;
+        const uint64_t start = (uint64_t)(t % tpr) * TILE;
         const uint64_t fill = min((uint64_t)cursor[p], pcap);
         if (start >= fill) continue;                    // block-uniform
         for (int k = threadIdx.x; k < nsub; k += 512) s_cnt[k] = 0;
         __syncthreads();
-        const int4* reg = pbuf + (size_t)p * (size_t)pcap;
-        int4 r[8];
-        uint32_t at[8];                                 // sub-bucket << 16 | rank in the tile (both < 2^13), ~0 = none
+        const R* reg = pbuf + (size_t)p * (size_t)pcap;
+        R r[ITEMS];
+        uint32_t at[ITEMS];                             // sub-bucket << 16 | rank in the tile (both < 2^13), ~0 = none
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
+        for (int k = 0; k < ITEMS; ++k) {
             const uint64_t i = start + (uint64_t)k * 512 + threadIdx.x;
             at[k] = HH_NONE32;
             if (i < fill) {
-                r[k] = hh_ld_stream(reg + i);
-                const uint32_t sub = hh_bucket_of(r[k], bucket_log) & (nsub - 1);
+                r[k] = hh_ld_rec(reg + i);
+                const uint32_t sub = hh_bucket_of(r[k], bucket_log, kbits) & (nsub - 1);
                 at[k] = (sub << 16) | atomicAdd(&s_cnt[sub], 1u);
             }
         }
@@ -599,16 +680,16 @@ hh_k_part_scatter2(const int4* __restrict__ pbuf, uint64_t pcap, const unsigned 
             if (s_cnt[k]) s_base[k] = atomicAdd(bfill + ((size_t)p << sub_log) + k, s_cnt[k]);
         const unsigned int n_tile = hh_tile_scan(s_cnt, nsub, s_wtot);
 #pragma unroll
-        for (int k = 0; k < 8; ++k)
+        for (int k = 0; k < ITEMS; ++k)
             if (at[k] != HH_NONE32) s_stage[s_cnt[at[k] >> 16] + (at[k] & 0xFFFFu)] = r[k];
         __syncthreads();
         // staged record e is number e - s_cnt[sub] of the tile's run in its sub-bucket
         for (unsigned int e = threadIdx.x; e < n_tile; e += 512) {
-            const int4 rec = s_stage[e];
-            const uint32_t sub = hh_bucket_of(rec, bucket_log) & (nsub - 1);
+            const R rec = s_stage[e];
+            const uint32_t sub = hh_bucket_of(rec, bucket_log, kbits) & (nsub - 1);
             const size_t b = ((size_t)p << sub_log) + sub;
             const uint64_t q = (uint64_t)boff[b] + s_base[sub] + (e - s_cnt[sub]);
-            if (q < n_out) out[q] = rec;
+            if (q < n_out) hh_rec_put(out + q, rec, kbits);
             else atomicExch(counters + 2, 6ull);
         }
         __syncthreads();
@@ -679,9 +760,9 @@ struct hh_bc_smem {
     int bucket;
 };
 
-template <typename K, int ITEMS>
+template <typename K, int ITEMS, typename R>
 __global__ void __launch_bounds__(HH_AGG_THREADS, 3)
-hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff, int nbuckets, uint64_t hot, int kbits,
+hh_k_bucket_count(const R* __restrict__ rec, const int64_t* __restrict__ boff, int nbuckets, uint64_t hot, int kbits,
                   uint32_t* __restrict__ compact, uint64_t compact_cap, unsigned long long* __restrict__ ctg_links,
                   unsigned long long* __restrict__ counters, unsigned long long* __restrict__ agg, uint32_t* __restrict__ fallback) {
     typedef hh_bc_smem<K, ITEMS> smem_t;
@@ -721,10 +802,10 @@ hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff
                 key[q] = ~(K)0;
                 pay[q] = 0;
                 if (l < m) {
-                    const int4 r = hh_ld_stream(rec + lo + c0 + l);
-                    key[q] = ((K)(uint32_t)r.x << kbits) | (K)(uint32_t)r.y;
-                    pay[q] = (uint32_t)l | (((uint32_t)r.w & 7u) << 11);
-                    sm.z[l] = (uint32_t)r.z;
+                    const R r = hh_ld_rec(rec + lo + c0 + l);
+                    key[q] = ((K)hh_rec_i(r, kbits) << kbits) | (K)hh_rec_j(r, kbits);
+                    pay[q] = (uint32_t)l | (hh_rec_flags(r) << 11);
+                    sm.z[l] = hh_rec_z(r);
                 }
             }
             typename smem_t::sort_t(sm.u.sort).Sort(key, pay, 0, 2 * kbits);
@@ -869,9 +950,11 @@ hh_k_bucket_count(const int4* __restrict__ rec, const int64_t* __restrict__ boff
 // so the keys of different buckets never meet and a batch may hold any number of them.
 #define HH_FB_BATCH (1 << 19)      // records per fallback batch: two 2^20-slot scratch tables of 42 MB at load <= 0.5
 
-// dst[pre[k] + r] = src[src_off[k] + r] for the nf listed buckets (pre = exclusive prefix of their record counts)
-__global__ void hh_k_gather_buckets(const int4* __restrict__ src, const int64_t* __restrict__ src_off, const int64_t* __restrict__ pre,
-                                    int nf, int4* __restrict__ dst) {
+// dst[pre[k] + r] = src[src_off[k] + r], as a wide record, for the nf listed buckets (pre = exclusive prefix of their
+// record counts)
+template <typename R>
+__global__ void hh_k_gather_buckets(const R* __restrict__ src, const int64_t* __restrict__ src_off, const int64_t* __restrict__ pre,
+                                    int nf, int kbits, int4* __restrict__ dst) {
     const int64_t total = pre[nf];
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
@@ -881,7 +964,7 @@ __global__ void hh_k_gather_buckets(const int4* __restrict__ src, const int64_t*
             if (pre[mid] <= i) lo = mid;
             else hi = mid - 1;
         }
-        dst[i] = hh_ld_stream(src + src_off[lo] + (i - pre[lo]));
+        hh_rec_put(dst + i, hh_ld_rec(src + src_off[lo] + (i - pre[lo])), kbits);
     }
 }
 
@@ -1334,6 +1417,8 @@ static int links_create_common(hh_ctx* ctx, int32_t n_key, const int64_t* key_le
     lk->n_src = frag_base ? n_src : n_key;
     lk->bin_size = bin_size;
     lk->flank_bp = flank_bp;
+    lk->kbits = 1;
+    while ((1ll << lk->kbits) < (int64_t)n_key) lk->kbits++;
     int rc = HH_OK;
     do {
         if ((rc = hh_dmalloc(&lk->d_len, n_key)) != HH_OK) break;
@@ -1405,14 +1490,23 @@ static int links_env_int(const char* name, int dflt) {
     return (v && *v) ? atoi(v) : dflt;
 }
 
-// a new set of partition regions sized for `n_rec` more records
-static int links_new_partset(hh_links* lk, int64_t n_rec) {
+// whether records of stream indices below `stream_end` can take the narrow format (see "partition records")
+static bool links_narrow(const hh_links* lk, int64_t stream_end) {
+    return lk->kbits <= HH_NREC_KBITS && stream_end <= HH_NREC_ZEND;
+}
+
+// a new set of partition regions sized for `n_rec` more records, ending at stream index `stream_end`
+static int links_new_partset(hh_links* lk, int64_t n_rec, int64_t stream_end) {
     const int npart = 1 << lk->npart_log;
     hh_partset ps;
     memset(&ps, 0, sizeof(ps));
     ps.pcap = (uint64_t)((double)n_rec / npart * 1.5) + 4096;
     ps.sized_for = n_rec;
-    HH_CHECK(hh_ws_alloc(lk->ctx, &ps.buf, (size_t)npart * (size_t)ps.pcap));
+    ps.narrow = links_narrow(lk, stream_end);
+    const size_t bytes = ps.narrow ? sizeof(hh_nrec) : sizeof(int4);
+    unsigned char* buf = nullptr;
+    HH_CHECK(hh_ws_alloc(lk->ctx, &buf, (size_t)npart * (size_t)ps.pcap * bytes));
+    ps.buf = buf;
     int rc = hh_dmalloc(&ps.cursor, (size_t)npart);
     if (rc != HH_OK) {
         hh_ws_free(lk->ctx, ps.buf);
@@ -1420,6 +1514,7 @@ static int links_new_partset(hh_links* lk, int64_t n_rec) {
     }
     HH_CUDA(cudaMemsetAsync(ps.cursor, 0, (size_t)npart * sizeof(unsigned long long), lk->ctx->stream));
     lk->psets.push_back(ps);
+    lk->set_bytes.push_back((int32_t)bytes);
     return HH_OK;
 }
 
@@ -1447,8 +1542,8 @@ static int links_size_spill(hh_links* lk) {
 }
 
 // first records of the stream: direct hash table or partition-then-aggregate.  `total` = records the caller is about to
-// stream in this call (the sizing of the partition regions)
-static int links_choose_mode(hh_links* lk, int64_t total) {
+// stream in this call (the sizing of the partition regions), from stream index `stream_offset`
+static int links_choose_mode(hh_links* lk, int64_t total, int64_t stream_offset) {
     if (lk->mode) return HH_OK;
     const int want = links_env_int("HH_LINKS_PARTITION", -1);          // 0 = never, 1 = always (contig mode), -1 = by size
     const bool can = lk->d_fbase == nullptr && lk->d_keys == nullptr;
@@ -1464,10 +1559,27 @@ static int links_choose_mode(hh_links* lk, int64_t total) {
     lk->npart_log = links_env_int("HH_LINKS_NPART_LOG", lg);
     if (lk->npart_log < 1) lk->npart_log = 1;
     if (lk->npart_log > 10) lk->npart_log = 10;
-    HH_CHECK(links_new_partset(lk, total));
+    HH_CHECK(links_new_partset(lk, total, stream_offset + total));
     HH_CHECK(links_size_spill(lk));
     HH_CHECK(hh_dmalloc(&lk->d_spill_cursor, 1));
     HH_CUDA(cudaMemsetAsync(lk->d_spill_cursor, 0, sizeof(unsigned long long), lk->ctx->stream));
+    return HH_OK;
+}
+
+// records -> the regions of the last partition set, whose records are R
+template <typename R>
+static int links_launch_scatter(hh_links* lk, R* pbuf, const int4* d_rec, int64_t n_rec, int64_t stream_offset) {
+    hh_ctx* ctx = lk->ctx;
+    auto kernel = hh_k_part_scatter<R>;
+    const int64_t tiles = (n_rec + hh_scatter_tile<R>() - 1) / hh_scatter_tile<R>();
+    int grid = 0;
+    HH_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HH_STAGE_SMEM));
+    HH_CHECK(hh_resident_grid(ctx, kernel, 512, HH_STAGE_SMEM, &grid));
+    grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, grid));
+    const hh_partset& ps = lk->psets.back();
+    HH_LAUNCH(ctx, kernel, grid, 512, HH_STAGE_SMEM, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank, lk->d_nx,
+              lk->flank_bp, lk->npart_log, lk->kbits, pbuf, ps.pcap, ps.cursor, lk->d_spill, lk->spill_cap, lk->d_spill_cursor,
+              lk->d_counters);
     return HH_OK;
 }
 
@@ -1475,16 +1587,9 @@ static int links_launch_insert(hh_links* lk, const int4* d_rec, int64_t n_rec, i
                                const uint32_t* d_pos = nullptr) {
     hh_ctx* ctx = lk->ctx;
     if (lk->mode == 2 && d_pos == nullptr) {
-        const int64_t tiles = (n_rec + HH_PART_TILE - 1) / HH_PART_TILE;
-        int grid = 0;
-        HH_CUDA(cudaFuncSetAttribute(hh_k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HH_STAGE_SMEM));
-        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter, 512, HH_STAGE_SMEM, &grid));
-        grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, grid));
         const hh_partset& ps = lk->psets.back();
-        HH_LAUNCH(ctx, hh_k_part_scatter, grid, 512, HH_STAGE_SMEM, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len, lk->d_rank, lk->d_nx,
-                  lk->flank_bp, lk->npart_log, ps.buf, ps.pcap, ps.cursor, lk->d_spill, lk->spill_cap, lk->d_spill_cursor,
-                  lk->d_counters);
-        return HH_OK;
+        return ps.narrow ? links_launch_scatter(lk, reinterpret_cast<hh_nrec*>(ps.buf), d_rec, n_rec, stream_offset)
+                         : links_launch_scatter(lk, reinterpret_cast<int4*>(ps.buf), d_rec, n_rec, stream_offset);
     }
     HH_CHECK(links_need_table(lk));
     HH_LAUNCH(ctx, hh_k_links_insert, links_grid(ctx, n_rec), 256, 0, d_rec, n_rec, (uint32_t)stream_offset, lk->n_ctg, lk->d_len,
@@ -1493,11 +1598,13 @@ static int links_launch_insert(hh_links* lk, const int4* d_rec, int64_t n_rec, i
     return HH_OK;
 }
 
-// partitioned mode: a call that would outgrow the current set (sized for the first call) gets a set of its own
-static int links_part_room(hh_links* lk, int64_t n_rec) {
+// partitioned mode: a call that would outgrow the current set (sized for the first call), or put a stream index beyond
+// the narrow format into a narrow set, gets a set of its own
+static int links_part_room(hh_links* lk, int64_t n_rec, int64_t stream_offset) {
     hh_partset& ps = lk->psets.back();
-    if (ps.sent > 0 && ps.sent + n_rec > ps.sized_for + ps.sized_for / 8) {
-        HH_CHECK(links_new_partset(lk, n_rec));
+    const bool outgrown = ps.sent + n_rec > ps.sized_for + ps.sized_for / 8;
+    if (ps.sent > 0 && (outgrown || (ps.narrow && !links_narrow(lk, stream_offset + n_rec)))) {
+        HH_CHECK(links_new_partset(lk, n_rec, stream_offset + n_rec));
         lk->psets.back().sent = n_rec;
         return links_size_spill(lk);
     }
@@ -1528,8 +1635,8 @@ extern "C" int hh_links_add_async(hh_links* lk, const int32_t* rec_dev, int64_t 
     HH_REQUIRE(((uintptr_t)rec_dev & 15) == 0, HH_ERR_ARG, "hh_links_add: records must be 16-byte aligned");
     if (n_rec == 0) return HH_OK;
     HH_CUDA(cudaSetDevice(lk->ctx->device));
-    HH_CHECK(links_choose_mode(lk, n_rec));
-    if (lk->mode == 2) HH_CHECK(links_part_room(lk, n_rec));
+    HH_CHECK(links_choose_mode(lk, n_rec, stream_offset));
+    if (lk->mode == 2) HH_CHECK(links_part_room(lk, n_rec, stream_offset));
     HH_CHECK(links_launch_insert(lk, reinterpret_cast<const int4*>(rec_dev), n_rec, stream_offset));
     lk->n_records += n_rec;
     lk->since_known += n_rec;
@@ -1549,8 +1656,8 @@ extern "C" int hh_links_add(hh_links* lk, const int32_t* rec, int64_t n_rec, int
     hh_ctx* ctx = lk->ctx;
     HH_CUDA(cudaSetDevice(ctx->device));
     const int64_t CH = HH_ADD_CHUNK;
-    HH_CHECK(links_choose_mode(lk, n_rec));
-    if (lk->mode == 2) HH_CHECK(links_part_room(lk, n_rec));
+    HH_CHECK(links_choose_mode(lk, n_rec, stream_offset));
+    if (lk->mode == 2) HH_CHECK(links_part_room(lk, n_rec, stream_offset));
     if (mem == HH_MEM_DEVICE) {
         HH_REQUIRE(((uintptr_t)rec & 15) == 0, HH_ERR_ARG, "hh_links_add: records must be 16-byte aligned");
         HH_CHECK(links_add_chunks(lk, reinterpret_cast<const int4*>(rec), nullptr, n_rec, stream_offset));
@@ -1613,27 +1720,56 @@ static uint64_t links_hot_records(int64_t n_used, int bucket_log) {
 
 // hh_k_bucket_count for keys of 2 kbits bits: 32-bit keys in chunks of 2048 records, 64-bit keys in chunks of 1280 (the
 // shared memory of three CTAs per SM)
-template <typename K, int ITEMS>
-static int links_bucket_count(hh_links* lk, const int4* rec, const int64_t* boff, int nb, uint64_t hot, int kbits, uint32_t* compact,
+template <typename K, int ITEMS, typename R>
+static int links_bucket_count(hh_links* lk, const void* rec, const int64_t* boff, int nb, uint64_t hot, int kbits, uint32_t* compact,
                               uint64_t compact_cap, unsigned long long* agg, uint32_t* fallback) {
     hh_ctx* ctx = lk->ctx;
-    auto kernel = hh_k_bucket_count<K, ITEMS>;
+    auto kernel = hh_k_bucket_count<K, ITEMS, R>;
     const size_t smem = sizeof(hh_bc_smem<K, ITEMS>);
     HH_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int grid = 0;
     HH_CHECK(hh_resident_grid(ctx, kernel, HH_AGG_THREADS, smem, &grid));
-    HH_LAUNCH(ctx, kernel, grid, HH_AGG_THREADS, smem, rec, boff, nb, hot, kbits, compact, compact_cap, lk->d_ctg, lk->d_counters, agg,
+    HH_LAUNCH(ctx, kernel, grid, HH_AGG_THREADS, smem, reinterpret_cast<const R*>(rec), boff, nb, hot, kbits, compact, compact_cap, lk->d_ctg, lk->d_counters, agg,
               fallback);
     return HH_OK;
 }
 
-// Device memory of the finish for P records sent, U of them usable: the regions (24 B x P + 32 MB at 512 partitions) and
-// the spill list (2 B x P + 64 MB), the bucket buffer (16 B x U) and the compact staging list (36 B x U).  The regions and
-// the spill list are released before the staging list is allocated, so at most 8.7 GB is in use at once at the
-// benchmark's 200M records (U = 167M).  Released blocks stay in the context's workspace cache, which gives them back only
-// when an allocation fails, and the staging list does not fit the regions' block: the process holds all four, 14.0 GB,
-// where the partition step this replaced held 11.4 GB (regions, spill list, staging list, two 42 MB scratch tables).  A
-// fallback adds its gathered records (16 B each), which take the place of the bucket buffer, and two scratch tables.
+// the records of every partition set (and, with the first, the spill list) per bucket
+template <typename R>
+static int links_launch_hist(hh_links* lk, const hh_partset& ps, int64_t n_spill, int blog, unsigned int* bcnt) {
+    hh_ctx* ctx = lk->ctx;
+    auto kernel = hh_k_part_hist<R>;
+    int grid = 0;
+    HH_CHECK(hh_resident_grid(ctx, kernel, 512, 0, &grid));
+    const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
+    HH_LAUNCH(ctx, kernel, grid, 512, 0, reinterpret_cast<const R*>(ps.buf), ps.pcap, ps.cursor, lk->npart_log, lk->kbits, tpr,
+              lk->d_spill, n_spill, blog, bcnt);
+    return HH_OK;
+}
+
+// every record of a partition set (and, with the first, of the spill list) to its place in the bucket buffer `out` of D
+template <typename R, typename D>
+static int links_launch_scatter2(hh_links* lk, const hh_partset& ps, int64_t n_spill, int blog, const int64_t* boff, unsigned int* bfill,
+                                 void* out, uint64_t n_out) {
+    hh_ctx* ctx = lk->ctx;
+    auto kernel = hh_k_part_scatter2<R, D>;
+    int grid = 0;
+    const size_t smem = (size_t)HH_PART_TILE * sizeof(R);
+    HH_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    HH_CHECK(hh_resident_grid(ctx, kernel, 512, smem, &grid));
+    const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
+    HH_LAUNCH(ctx, kernel, grid, 512, smem, reinterpret_cast<const R*>(ps.buf), ps.pcap, ps.cursor, lk->npart_log, lk->kbits, tpr,
+              lk->d_spill, n_spill, blog, boff, bfill, reinterpret_cast<D*>(out), n_out, lk->d_counters);
+    return HH_OK;
+}
+
+// Device memory of the finish for P records sent, U of them usable, in the narrow format (wide: twice the first and the
+// third): the regions (12 B x P + 16 MB at 512 partitions) and the spill list (2 B x P + 64 MB), the bucket buffer
+// (8 B x U) and the compact staging list (36 B x U).  The regions and the spill list are released before the staging list
+// is allocated, so at most 7.4 GB is in use at once at the benchmark's 200M records (U = 167M).  Released blocks stay in
+// the context's workspace cache, which gives them back only when an allocation fails, and the staging list does not fit
+// the regions' block: the process holds all four, 10.2 GB (14.0 GB with wide records).  A fallback adds its gathered
+// records (16 B each), which take the place of the bucket buffer, and two scratch tables.
 static int links_finish_partitioned(hh_links* lk) {
     hh_ctx* ctx = lk->ctx;
     unsigned long long c[8];
@@ -1657,7 +1793,8 @@ static int links_finish_partitioned(hh_links* lk) {
     uint32_t *d_fallback = nullptr, *d_stage_compact = nullptr;  // the exact-size list is cut from the staging list
     int64_t* d_boff = nullptr;
     unsigned long long* d_agg = nullptr;
-    int4 *d_rec2 = nullptr, *d_fb_rec = nullptr;
+    unsigned char* d_rec2 = nullptr;                              // the bucket buffer: hh_nrec when narrow, else int4
+    int4* d_fb_rec = nullptr;
     int64_t* d_fb_off = nullptr;                                  // fallback: [nf] bucket offsets, [nf + 1] prefix of their records
     uint64_t* skeys[2] = {nullptr, nullptr};
     hh_slot* svals[2] = {nullptr, nullptr};
@@ -1668,36 +1805,34 @@ static int links_finish_partitioned(hh_links* lk) {
         HH_CHECK(hh_dmalloc(&d_boff, (size_t)nb + 1));
         HH_CHECK(hh_dmalloc(&d_fallback, (size_t)nb));
         HH_CHECK(hh_dmalloc(&d_agg, 4));
-        HH_CHECK(hh_ws_alloc(ctx, &d_rec2, (size_t)compact_cap));
+        const bool narrow = links_narrow(lk, lk->stream_end);
+        lk->bucket_bytes = narrow ? (int32_t)sizeof(hh_nrec) : (int32_t)sizeof(int4);
+        HH_CHECK(hh_ws_alloc(ctx, &d_rec2, (size_t)compact_cap * (size_t)lk->bucket_bytes));
         HH_CUDA(cudaMemsetAsync(d_bcnt, 0, (size_t)nb * sizeof(unsigned int), ctx->stream));
         HH_CUDA(cudaMemsetAsync(d_bfill, 0, (size_t)nb * sizeof(unsigned int), ctx->stream));
         HH_CUDA(cudaMemsetAsync(d_agg, 0, 4 * sizeof(unsigned long long), ctx->stream));
         // ---- buckets: records per bucket, dense offsets, every record to its bucket
-        int grid = 0, grid2 = 0;
-        HH_CHECK(hh_resident_grid(ctx, hh_k_part_hist, 512, 0, &grid));
-        HH_CUDA(cudaFuncSetAttribute(hh_k_part_scatter2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HH_STAGE_SMEM));
-        HH_CHECK(hh_resident_grid(ctx, hh_k_part_scatter2, 512, HH_STAGE_SMEM, &grid2));
         for (size_t k = 0; k < lk->psets.size(); ++k) {
             const hh_partset& ps = lk->psets[k];
-            const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
-            HH_LAUNCH(ctx, hh_k_part_hist, grid, 512, 0, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
-                      k == 0 ? (int64_t)n_spill : 0, blog, d_bcnt);
+            const int64_t ns = k == 0 ? (int64_t)n_spill : 0;
+            HH_CHECK(ps.narrow ? links_launch_hist<hh_nrec>(lk, ps, ns, blog, d_bcnt) : links_launch_hist<int4>(lk, ps, ns, blog, d_bcnt));
         }
         HH_CHECK(hh_exclusive_scan_i32(ctx, reinterpret_cast<const int*>(d_bcnt), d_boff, nb));
         for (size_t k = 0; k < lk->psets.size(); ++k) {
             const hh_partset& ps = lk->psets[k];
-            const int64_t tpr = (int64_t)((ps.pcap + HH_PART_TILE - 1) / HH_PART_TILE);
-            HH_LAUNCH(ctx, hh_k_part_scatter2, grid2, 512, HH_STAGE_SMEM, ps.buf, ps.pcap, ps.cursor, lk->npart_log, tpr, lk->d_spill,
-                      k == 0 ? (int64_t)n_spill : 0, blog, d_boff, d_bfill, d_rec2, compact_cap, lk->d_counters);
+            const int64_t ns = k == 0 ? (int64_t)n_spill : 0;
+            auto scatter2 = ps.narrow ? (narrow ? links_launch_scatter2<hh_nrec, hh_nrec> : links_launch_scatter2<hh_nrec, int4>)
+                                      : (narrow ? links_launch_scatter2<int4, hh_nrec> : links_launch_scatter2<int4, int4>);
+            HH_CHECK(scatter2(lk, ps, ns, blog, d_boff, d_bfill, d_rec2, compact_cap));
         }
         links_free_partsets(lk);                               // ordered on the stream behind scatter2
         HH_CHECK(hh_ws_alloc(ctx, &d_stage_compact, (size_t)compact_cap * HH_E_WORDS));
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 0, 0, sizeof(unsigned long long), ctx->stream));     // entry cursor
         HH_CUDA(cudaMemsetAsync(lk->d_counters + 3, 0, sizeof(unsigned long long), ctx->stream));     // nnz_flank
         // ---- every bucket in shared memory
-        int kbits = 1;                                         // key (i << kbits) | j
-        while ((1ll << kbits) < (int64_t)lk->n_ctg) kbits++;
-        auto count = 2 * kbits <= 32 ? links_bucket_count<uint32_t, 8> : links_bucket_count<uint64_t, 5>;
+        const int kbits = lk->kbits;                           // key (i << kbits) | j
+        auto count = narrow ? links_bucket_count<uint32_t, 8, hh_nrec>
+                            : 2 * kbits <= 32 ? links_bucket_count<uint32_t, 8, int4> : links_bucket_count<uint64_t, 5, int4>;
         HH_CHECK(count(lk, d_rec2, d_boff, nb, hot, kbits, d_stage_compact, compact_cap, d_agg, d_fallback));
         unsigned long long agg[4];
         HH_CUDA(cudaMemcpyAsync(agg, d_agg, sizeof(agg), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1733,7 +1868,12 @@ static int links_finish_partitioned(hh_links* lk) {
             HH_CUDA(cudaMemcpyAsync(d_fb_off, src_off.data(), (size_t)nf * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
             HH_CUDA(cudaMemcpyAsync(d_fb_off + nf, pre.data(), ((size_t)nf + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
             HH_CHECK(hh_ws_alloc(ctx, &d_fb_rec, (size_t)pre[nf]));
-            HH_LAUNCH(ctx, hh_k_gather_buckets, hh_grid(ctx, 8), 256, 0, d_rec2, d_fb_off, d_fb_off + nf, nf, d_fb_rec);
+            if (narrow)
+                HH_LAUNCH(ctx, hh_k_gather_buckets<hh_nrec>, hh_grid(ctx, 8), 256, 0, reinterpret_cast<const hh_nrec*>(d_rec2), d_fb_off,
+                          d_fb_off + nf, nf, kbits, d_fb_rec);
+            else
+                HH_LAUNCH(ctx, hh_k_gather_buckets<int4>, hh_grid(ctx, 8), 256, 0, reinterpret_cast<const int4*>(d_rec2), d_fb_off,
+                          d_fb_off + nf, nf, kbits, d_fb_rec);
             hh_ws_free(ctx, d_rec2);                           // ordered on the stream behind the gather
             for (int t = 0; t < 2; ++t) HH_CHECK(links_alloc_table(lk, scap, &skeys[t], &svals[t]));
             const int g = hh_grid(ctx, 8);
@@ -1776,6 +1916,14 @@ static int links_finish_partitioned(hh_links* lk) {
     lk->finished = true;
     lk->gen++;                  // the linked index of an earlier table does not apply
     lk->ordered = false;        // dict insertion order is restored by the first hh_links_fetch (links_order_list)
+    return HH_OK;
+}
+
+extern "C" int hh_links_record_bytes(hh_links* lk, int32_t* set_bytes, int32_t max_sets, int32_t* n_sets, int32_t* bucket_bytes) {
+    HH_REQUIRE(lk != nullptr && (max_sets <= 0 || set_bytes), HH_ERR_ARG, "hh_links_record_bytes: NULL argument");
+    for (int32_t k = 0; k < max_sets && k < (int32_t)lk->set_bytes.size(); ++k) set_bytes[k] = lk->set_bytes[k];
+    if (n_sets) *n_sets = (int32_t)lk->set_bytes.size();
+    if (bucket_bytes) *bucket_bytes = lk->bucket_bytes;
     return HH_OK;
 }
 

@@ -119,6 +119,16 @@ class LinkTable:
         check(load().hh_links_agg_info(self._h, C.byref(b), C.byref(s), C.byref(f)))
         return {"buckets": int(b.value), "smem_buckets": int(s.value), "fallback_buckets": int(f.value)}
 
+    def record_bytes(self) -> dict:
+        """Bytes per record of a partitioned count: ``sets``, one entry per partition set opened by the add calls, and
+        ``buckets``, the bucket buffer of the finish (0 before it).  8 is the narrow format (at most 65,536 contigs and
+        stream indices below 2^29), 16 the wide one; no sets and 0 for a table counted directly."""
+        n, b = C.c_int32(), C.c_int32()
+        check(load().hh_links_record_bytes(self._h, None, 0, C.byref(n), C.byref(b)))
+        sets = (C.c_int32 * max(1, n.value))()
+        check(load().hh_links_record_bytes(self._h, sets, n.value, C.byref(n), C.byref(b)))
+        return {"sets": [int(x) for x in sets[:n.value]], "buckets": int(b.value)}
+
     # -- results ---------------------------------------------------------------------------
     def fetch(self, pinned: bool = False) -> dict:
         """Arrays of nnz_full entries in full_link_dict insertion order.  ``pinned=True`` returns views of

@@ -112,6 +112,11 @@ int hh_links_finish(hh_links* lk, hh_links_info* info);
  * number of hash buckets, those counted in a shared-memory table, and those counted by the global-table fallback
  * (too many records or distinct pairs for shared memory).  All 0 for a table counted directly.  Any pointer may be NULL. */
 int hh_links_agg_info(hh_links* lk, int64_t* buckets, int64_t* smem_buckets, int64_t* fallback_buckets);
+/* bytes per record of the partitioned count: of every partition set opened so far, in order (the first max_sets of them
+ * to set_bytes, their number to *n_sets), and of the bucket buffer of its finish (*bucket_bytes, 0 before the finish).
+ * 8 = the narrow format (at most 65,536 objects and stream indices below 2^29), 16 = the wide one.  No sets and 0 for a
+ * table counted directly.  set_bytes may be NULL when max_sets <= 0, the other pointers always. */
+int hh_links_record_bytes(hh_links* lk, int32_t* set_bytes, int32_t max_sets, int32_t* n_sets, int32_t* bucket_bytes);
 
 /* full_link_dict / flank_link_dict / HT_link_dict as parallel arrays of nnz_full entries in
  * full_link_dict insertion order (1649).  key_i/key_j: contig ids with name(key_i) < name(key_j).
