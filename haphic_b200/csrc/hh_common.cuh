@@ -191,6 +191,41 @@ __device__ __forceinline__ float4 hh_ld_stream_f4(const float4* p) {
     return r;
 }
 
+// Exclusive prefix, in place, of the n <= 8 x 512 counts c[] of a tile, by its 512 threads; returns their sum.  s_wtot is
+// shared scratch of 16 words.  Barriers on entry (c[] is complete) and on exit (the prefix is visible).
+__device__ __forceinline__ unsigned int hh_tile_scan(unsigned int* c, int n, unsigned int* s_wtot) {
+    const int lane = threadIdx.x & 31, wv = threadIdx.x >> 5;
+    const int per = (n + 511) >> 9, lo = threadIdx.x * per;
+    __syncthreads();
+    unsigned int sum = 0;
+    for (int k = 0; k < per; ++k)
+        if (lo + k < n) sum += c[lo + k];
+    unsigned int incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned int t = __shfl_up_sync(HH_FULL_MASK, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_wtot[wv] = incl;
+    __syncthreads();
+    unsigned int run = incl - sum, all = 0;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+        const unsigned int t = s_wtot[k];
+        run += (k < wv) ? t : 0u;
+        all += t;
+    }
+    for (int k = 0; k < per; ++k) {
+        if (lo + k < n) {
+            const unsigned int t = c[lo + k];
+            c[lo + k] = run;
+            run += t;
+        }
+    }
+    __syncthreads();
+    return all;
+}
+
 // CTAs of `kernel` (at `threads` threads and `smem` bytes of dynamic shared memory) that the GPU holds at once: the grid of
 // a persistent kernel whose CTAs each loop over a fixed share of the work, so that none waits for another to exit
 template <typename K>

@@ -22,7 +22,7 @@ enum { HH_E_I, HH_E_J, HH_E_FULL, HH_E_FLANK, HH_E_FIRST_FULL, HH_E_FIRST_FLANK,
 // the two ends lie on two different contigs (ul_parent) of one ultra-long-read path (add_flank_and_full_links_based_on_ul,
 // 1936-1985), then -- when hap != NULL and the two ends lie on different haplotypes -- x - x * w with two roundings
 // (reduce_inter_hap_HiC_links, 695-707).  Returns false when the entry is not in the (reduced) flank_link_dict: no flank
-// link, or reduced to exactly 0.  hh_k_touch and hh_k_mat_scatter both decide through this one function, so pattern,
+// link, or reduced to exactly 0.  hh_k_touch and hh_k_mat_group both decide through this one function, so pattern,
 // values and first-seen indices cannot disagree; doubling never makes a value 0, so the index pass may leave ul_path NULL.
 __device__ __forceinline__ bool hh_flank_value(const uint32_t* __restrict__ p, const unsigned long long* __restrict__ ctg_tot,
                                                int normalize, const int32_t* __restrict__ hap, double w,

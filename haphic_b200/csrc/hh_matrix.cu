@@ -50,27 +50,190 @@ __global__ void hh_k_mat_self_loops(int n, const int64_t* __restrict__ colptr, i
     val[q] = 1.0f;
 }
 
-// every passing entry to its two columns; the order of rows inside a column is left unspecified
-__global__ void hh_k_mat_scatter(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
-                                 const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap,
-                                 double w, const int32_t* __restrict__ ul_path, const int32_t* __restrict__ ul_parent,
-                                 const int64_t* __restrict__ colptr, int* __restrict__ cursor,
-                                 int32_t* __restrict__ row, float* __restrict__ val) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += stride) {
-        const uint32_t* p = compact + e * HH_E_WORDS;
-        if (p[HH_E_FLANK] == 0) continue;
-        const int ii = index[p[HH_E_I]], jj = index[p[HH_E_J]];
-        if (ii < 0 || jj < 0) continue;                 // 329-330
-        double x;
-        if (!hh_flank_value(p, ctg_tot, normalize, hap, w, ul_path, ul_parent, &x)) continue;
-        const float v = (float)x;                      // coo_matrix(dtype=float32) (368)
-        int64_t q = colptr[jj] + atomicAdd(cursor + jj, 1);    // (row ii, col jj)
-        row[q] = ii;
-        val[q] = v;
-        q = colptr[ii] + atomicAdd(cursor + ii, 1);            // diagonal symmetry (351-353)
-        row[q] = jj;
-        val[q] = v;
+// ---------------------------------------------------------------------------------------------
+// Placement of the passing entries, in two passes through a staging list laid out like the CSC.  The matrix columns are
+// cut into groups of C = 2^cbits consecutive columns (hh_mat_cbits: at most 4096 groups).  A staged half-entry is 8 bytes,
+// {row << cbits | column - g·C, fp32 value}, and group g's staging run is the part of its CSC extent that the self loops
+// leave, [colptr[g·C] + sl·(columns of g), colptr[(g+1)·C]).
+//   hh_k_mat_group   tiles of compact entries: both halves of every passing entry, counted per group in shared memory,
+//                    one global reservation per (tile, group), stored run by run from a staged copy of the tile
+//   hh_k_mat_chunks  one CTA: the groups' staging cursors and the list of chunks (at most HH_MAT_CHUNK staged records,
+//                    inside one group)
+//   hh_k_mat_place   persistent CTAs, one chunk at a time: a counting sort of the chunk over its group's columns in
+//                    shared memory, one cursor atomic per (chunk, column), rows and values stored in column runs
+// Few groups keep the staging runs long; chunks of 8192 records keep the placement's write front at one group's columns.
+// ---------------------------------------------------------------------------------------------
+#define HH_MAT_TILE 4096           // compact entries per tile of hh_k_mat_group (512 threads x 8): 2 x 4096 half-entries
+#define HH_MAT_CHUNK 8192          // staged records per chunk of hh_k_mat_place (512 threads x 16)
+#define HH_MAT_MAX_N (1 << 22)     // bits(n) + cbits <= 32: the staged word holds the row and the column in the group
+
+struct hh_mat_chunk {
+    long long start;               // first staged record
+    int len;                       // records, 1 .. HH_MAT_CHUNK
+    int group;
+};
+
+// columns per group: C = 2^cbits with cbits = max(8, bits(n) - 12), so at most 4096 groups
+static int hh_mat_cbits(int n) {
+    int bits = 0;
+    while (((int64_t)1 << bits) < n) ++bits;
+    return std::max(8, bits - 12);
+}
+
+// shared memory of hh_k_mat_group: the staged tile, the group of every staged record, then per group its reservation
+// and count
+static size_t hh_mat_group_smem(int ngroups) {
+    return (size_t)2 * HH_MAT_TILE * (sizeof(uint2) + sizeof(uint16_t)) + (size_t)ngroups * (sizeof(unsigned long long) + sizeof(unsigned int));
+}
+
+__global__ void __launch_bounds__(512, 2)
+hh_k_mat_group(const uint32_t* __restrict__ compact, int64_t nnz, const int32_t* __restrict__ index,
+               const unsigned long long* __restrict__ ctg_tot, int normalize, const int32_t* __restrict__ hap, double w,
+               const int32_t* __restrict__ ul_path, const int32_t* __restrict__ ul_parent, int cbits, int ngroups,
+               unsigned long long* __restrict__ gcur, uint2* __restrict__ stage) {
+    constexpr int ITEMS = HH_MAT_TILE / 512;
+    extern __shared__ uint2 s_mat_mem[];
+    uint2* s_stage = s_mat_mem;                                               // the tile's half-entries, ordered by group
+    uint16_t* s_grp = reinterpret_cast<uint16_t*>(s_stage + 2 * HH_MAT_TILE);  // the group of each staged one
+    unsigned long long* s_base = reinterpret_cast<unsigned long long*>(s_grp + 2 * HH_MAT_TILE);
+    unsigned int* s_cnt = reinterpret_cast<unsigned int*>(s_base + ngroups);  // half-entries per group, then their prefix
+    __shared__ unsigned int s_wtot[16];
+    const uint32_t cmask = (1u << cbits) - 1u;
+    const int64_t tiles = (nnz + HH_MAT_TILE - 1) / HH_MAT_TILE;
+    for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+        for (int k = threadIdx.x; k < ngroups; k += 512) s_cnt[k] = 0;
+        __syncthreads();
+        // The words of the tile's entries are loaded together, then the matrix indices of their ends; ii[k] = -1 marks an
+        // entry that does not pass.  Shared cursors over the scanned counts give the staged places, so no rank is held.
+        int ii[ITEMS], jj[ITEMS];
+        float v[ITEMS];
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k) {
+            const int64_t e = t * HH_MAT_TILE + (int64_t)k * 512 + threadIdx.x;
+            ii[k] = -1;
+            if (e < nnz) {
+                const uint32_t* p = compact + e * HH_E_WORDS;
+                const uint32_t fl = p[HH_E_FLANK], ci = p[HH_E_I], cj = p[HH_E_J];
+                if (fl) {
+                    ii[k] = (int)ci;
+                    jj[k] = (int)cj;
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k) {
+            if (ii[k] < 0) continue;
+            ii[k] = index[ii[k]];
+            jj[k] = index[jj[k]];
+        }
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k) {
+            if (ii[k] < 0 || jj[k] < 0) {                // 329-330
+                ii[k] = -1;
+                continue;
+            }
+            double x;
+            if (!hh_flank_value(compact + (t * HH_MAT_TILE + (int64_t)k * 512 + threadIdx.x) * HH_E_WORDS, ctg_tot, normalize, hap,
+                                w, ul_path, ul_parent, &x)) {
+                ii[k] = -1;
+                continue;
+            }
+            v[k] = (float)x;                             // coo_matrix(dtype=float32) (368)
+            // (row ii, column jj) and its diagonal mirror (351-353)
+            atomicAdd(&s_cnt[jj[k] >> cbits], 1u);
+            atomicAdd(&s_cnt[ii[k] >> cbits], 1u);
+        }
+        __syncthreads();
+        for (int k = threadIdx.x; k < ngroups; k += 512)
+            if (s_cnt[k]) s_base[k] = atomicAdd(gcur + k, (unsigned long long)s_cnt[k]);
+        const unsigned int n_tile = hh_tile_scan(s_cnt, ngroups, s_wtot);
+        // staged record e of group g goes to s_base[g] + e; s_cnt becomes the staging cursors
+        for (int k = threadIdx.x; k < ngroups; k += 512) s_base[k] -= s_cnt[k];
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k) {
+            if (ii[k] < 0) continue;
+            const uint32_t a = (uint32_t)ii[k], b = (uint32_t)jj[k];
+            const unsigned int qa = atomicAdd(&s_cnt[b >> cbits], 1u);
+            s_stage[qa] = make_uint2(a << cbits | (b & cmask), __float_as_uint(v[k]));
+            s_grp[qa] = (uint16_t)(b >> cbits);
+            const unsigned int qb = atomicAdd(&s_cnt[a >> cbits], 1u);
+            s_stage[qb] = make_uint2(b << cbits | (a & cmask), __float_as_uint(v[k]));
+            s_grp[qb] = (uint16_t)(a >> cbits);
+        }
+        __syncthreads();
+        for (unsigned int e = threadIdx.x; e < n_tile; e += 512) stage[s_base[s_grp[e]] + e] = s_stage[e];
+        __syncthreads();
+    }
+}
+
+// One CTA of 512 threads: gcur[g] = the start of group g's staging run, and the chunk list (*n_chunks chunks, those of
+// one group consecutive)
+__global__ void __launch_bounds__(512)
+hh_k_mat_chunks(const int64_t* __restrict__ colptr, int n, int cbits, int ngroups, int sl, unsigned long long* __restrict__ gcur,
+                hh_mat_chunk* __restrict__ chunk, unsigned int* __restrict__ n_chunks) {
+    __shared__ unsigned int s_off[4096];                // chunks per group, then their exclusive prefix
+    __shared__ unsigned int s_wtot[16];
+    for (int g = threadIdx.x; g < ngroups; g += 512) {
+        const int lo = g << cbits, hi = min(n, lo + (1 << cbits));
+        const int64_t s = colptr[lo] + (int64_t)sl * (hi - lo);
+        gcur[g] = (unsigned long long)s;
+        s_off[g] = (unsigned int)((colptr[hi] - s + HH_MAT_CHUNK - 1) / HH_MAT_CHUNK);
+    }
+    const unsigned int total = hh_tile_scan(s_off, ngroups, s_wtot);
+    for (unsigned int c = threadIdx.x; c < total; c += 512) {
+        int g = 0;                                      // the last group whose chunks start at or before c
+        for (int step = 2048; step > 0; step >>= 1)
+            if (g + step < ngroups && s_off[g + step] <= c) g += step;
+        const int lo = g << cbits, hi = min(n, lo + (1 << cbits));
+        const int64_t s = colptr[lo] + (int64_t)sl * (hi - lo) + (int64_t)(c - s_off[g]) * HH_MAT_CHUNK;
+        chunk[c] = hh_mat_chunk{s, (int)min((int64_t)HH_MAT_CHUNK, colptr[hi] - s), g};
+    }
+    if (threadIdx.x == 0) *n_chunks = total;
+}
+
+__global__ void __launch_bounds__(512, 2)
+hh_k_mat_place(const uint2* __restrict__ stage, const hh_mat_chunk* __restrict__ chunk, const unsigned int* __restrict__ n_chunks,
+               int cbits, const int64_t* __restrict__ colptr, int* __restrict__ cursor, int32_t* __restrict__ row,
+               float* __restrict__ val) {
+    constexpr int ITEMS = HH_MAT_CHUNK / 512;
+    extern __shared__ uint2 s_mat_mem[];
+    uint2* s_rec = s_mat_mem;                           // the chunk, ordered by column
+    __shared__ unsigned int s_cnt[1024];                // records per column, their prefix, then the placement cursors
+    __shared__ long long s_base[1024];                  // CSC position of the column's run, minus its first staged slot
+    __shared__ unsigned int s_wtot[16];
+    const int ncol = 1 << cbits;
+    const uint32_t cmask = (uint32_t)ncol - 1u;
+    const unsigned int total = *n_chunks;
+    for (unsigned int c = blockIdx.x; c < total; c += gridDim.x) {
+        const hh_mat_chunk ch = chunk[c];
+        for (int k = threadIdx.x; k < ncol; k += 512) s_cnt[k] = 0;
+        __syncthreads();
+        uint2 r[ITEMS];
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k)
+            if (k * 512 + (int)threadIdx.x < ch.len) r[k] = stage[ch.start + k * 512 + threadIdx.x];
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k)
+            if (k * 512 + (int)threadIdx.x < ch.len) atomicAdd(&s_cnt[r[k].x & cmask], 1u);
+        __syncthreads();
+        const int col0 = ch.group << cbits;
+        for (int k = threadIdx.x; k < ncol; k += 512)
+            if (s_cnt[k]) s_base[k] = colptr[col0 + k] + atomicAdd(cursor + col0 + k, (int)s_cnt[k]);
+        hh_tile_scan(s_cnt, ncol, s_wtot);
+        for (int k = threadIdx.x; k < ncol; k += 512) s_base[k] -= s_cnt[k];
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k)
+            if (k * 512 + (int)threadIdx.x < ch.len) s_rec[atomicAdd(&s_cnt[r[k].x & cmask], 1u)] = r[k];
+        __syncthreads();
+        for (int e = threadIdx.x; e < ch.len; e += 512) {
+            const uint2 x = s_rec[e];
+            const long long q = s_base[x.x & cmask] + e;
+            row[q] = (int32_t)(x.x >> cbits);
+            val[q] = __uint_as_float(x.y);
+        }
+        __syncthreads();
     }
 }
 
@@ -128,12 +291,18 @@ extern "C" int hh_matrix_from_links_ex(hh_links* lk, const uint8_t* keep, const 
                "hh_matrix_from_links: tail lists an id that is dropped, linked, repeated or out of range");
     const int n = n_linked + n_tail;
     HH_REQUIRE(n > 0, HH_ERR_ARG, "hh_matrix_from_links: empty fragment set");
+    HH_REQUIRE(n <= HH_MAT_MAX_N, HH_ERR_ARG, "hh_matrix_from_links: %d fragments in the matrix, at most %d are supported", n,
+               HH_MAT_MAX_N);
     const int sl = add_self_loops ? 1 : 0;
     const int64_t nnz = 2 * n_pass + (int64_t)sl * n;      // known before any sync: the matrix is allocated up front
     int* d_err = reinterpret_cast<int*>(ctx->d_scratch + 10);
     int32_t* d_tail = nullptr;
     int32_t* d_ul = nullptr;
     int* d_cnt = nullptr;
+    uint2* d_stage = nullptr;
+    unsigned long long* d_gcur = nullptr;
+    hh_mat_chunk* d_chunk = nullptr;
+    unsigned int* d_nchunk = nullptr;
     hh_matrix* m = nullptr;
     int rc = [&]() -> int {
         HH_CHECK(matrix_alloc(ctx, n, nnz, &m));
@@ -163,11 +332,25 @@ extern "C" int hh_matrix_from_links_ex(hh_links* lk, const uint8_t* keep, const 
             HH_CUDA(cudaMemcpyAsync(d_ul + n_ctg, ul_parent, (size_t)n_ctg * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
         }
         if (n_pass) {
-            int gridc = 0;
-            HH_CHECK(hh_resident_grid(ctx, hh_k_mat_scatter, 256, 0, &gridc));
-            gridc = (int)std::min<int64_t>((nnz_c + 255) / 256, gridc);
-            HH_LAUNCH(ctx, hh_k_mat_scatter, gridc, 256, 0, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks, d_hap,
-                      w, d_ul, d_ul ? d_ul + n_ctg : nullptr, m->d_colptr, d_cursor, m->d_row, m->d_val);
+            const int cbits = hh_mat_cbits(n), ngroups = (n + (1 << cbits) - 1) >> cbits;
+            const int64_t max_chunks = (nnz + HH_MAT_CHUNK - 1) / HH_MAT_CHUNK + ngroups;
+            HH_CHECK(hh_ws_alloc(ctx, &d_stage, (size_t)nnz));
+            HH_CHECK(hh_dmalloc(&d_gcur, (size_t)ngroups));
+            HH_CHECK(hh_dmalloc(&d_chunk, (size_t)max_chunks));
+            HH_CHECK(hh_dmalloc(&d_nchunk, 1));
+            HH_LAUNCH(ctx, hh_k_mat_chunks, 1, 512, 0, m->d_colptr, n, cbits, ngroups, sl, d_gcur, d_chunk, d_nchunk);
+            const size_t smem1 = hh_mat_group_smem(ngroups), smem2 = (size_t)HH_MAT_CHUNK * sizeof(uint2);
+            int grid = 0;
+            HH_CUDA(cudaFuncSetAttribute(hh_k_mat_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+            HH_CHECK(hh_resident_grid(ctx, hh_k_mat_group, 512, smem1, &grid));
+            grid = (int)std::min<int64_t>((nnz_c + HH_MAT_TILE - 1) / HH_MAT_TILE, grid);
+            HH_LAUNCH(ctx, hh_k_mat_group, grid, 512, smem1, compact, nnz_c, d_index, hh_links_ctg_totals(lk), normalize_by_nlinks,
+                      d_hap, w, d_ul, d_ul ? d_ul + n_ctg : nullptr, cbits, ngroups, d_gcur, d_stage);
+            HH_CUDA(cudaFuncSetAttribute(hh_k_mat_place, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+            HH_CHECK(hh_resident_grid(ctx, hh_k_mat_place, 512, smem2, &grid));
+            grid = (int)std::min<int64_t>(max_chunks, grid);
+            HH_LAUNCH(ctx, hh_k_mat_place, grid, 512, smem2, d_stage, d_chunk, d_nchunk, cbits, m->d_colptr, d_cursor, m->d_row,
+                      m->d_val);
         }
         HH_CUDA(cudaMemcpyAsync(ctx->h_scratch + 10, d_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         HH_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -180,6 +363,10 @@ extern "C" int hh_matrix_from_links_ex(hh_links* lk, const uint8_t* keep, const 
     hh_dfree(d_tail);
     hh_dfree(d_ul);
     hh_dfree(d_cnt);
+    hh_ws_free(ctx, d_stage);
+    hh_dfree(d_gcur);
+    hh_dfree(d_chunk);
+    hh_dfree(d_nchunk);
     if (rc != HH_OK) {
         hh_matrix_destroy(m);
         return rc;

@@ -173,7 +173,8 @@ int hh_links_destroy(hh_links* lk);
  *     restricted to `keep` (327-349); index[c] = -1 otherwise; *n_linked = len(frags_in_dict).
  *   hh_matrix_from_links: builds the symmetric fp32 matrix, with self loops = 1 when add_self_loops (351-364);
  *     `tail[n_tail]` lists the kept-but-unlinked contig ids in the order they get the following
- *     indices.  normalize_by_nlinks != 0 applies links / sqrt(tot_i * tot_j) first (718-724).
+ *     indices.  normalize_by_nlinks != 0 applies links / sqrt(tot_i * tot_j) first (718-724).  A matrix of more than
+ *     2^22 fragments (n_linked + n_tail) is refused with HH_ERR_ARG.
  */
 int hh_links_linked_index(hh_links* lk, const uint8_t* keep, int32_t* index, int32_t* n_linked);
 int hh_matrix_from_links(hh_links* lk, const uint8_t* keep, const int32_t* tail, int32_t n_tail,
